@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — milli query-time scoring path on B200 (contract: the task's ④; SURVEY.md §8(d)).
+"""bench.py — milli query-time scoring path on H100 (SURVEY.md §8(d)).
 
 Default workload = cfg 3, the configuration BASELINE.json's metric is quoted on:
   synthetic "hackernews" corpus, 10 M docs x 1 searchable field, 1.5 M-word Zipf vocabulary, default criteria, limit 20,
@@ -12,7 +12,8 @@ One *step* = one such batch through b200_search_batch (mode 2).  `--mode keyword
             overlap there): every host<->device round trip's first..last kernel + the term-derivation sweep + the vector stage
   e2e       queries/sec through the C ABI with HOST buffers: wall clock around the K calls (host-side ranking-rule control flow,
             every H2D/D2H copy, all synchronisation, the hybrid merge)
-  roofline  dominant kernel (largest accumulated CUDA-event time): algorithmic bytes (or flops) / its event time vs the measured peak
+  roofline  dominant kernel (largest accumulated CUDA-event time): algorithmic bytes (or flops) / its event time vs the peak
+            (MEASURED_PEAKS.json when present, else the H100 SXM data sheet)
   cpu_baseline / --impl reference   the CPU oracle ("port": C++ restatement of milli; the Rust reference cannot be built here) on a
             bounded sample of the same queries, fixed thread count, with the latency distribution and a searchCutoffMs-clamped figure
   parity    ALL queries of one timed batch against the oracle: docids, ScoreDetails rank tuples, candidate counts (keyword,
@@ -43,7 +44,7 @@ def log(*a):
 
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    out = {"hbm": (6650.0, "fallback"), "tensor": (1590.0, "fallback")}
+    out = {"hbm": (3350.0, "H100 SXM data sheet"), "tensor": (989.0, "H100 SXM data sheet, dense fp16")}
     if os.path.exists(p):
         try:
             d = json.load(open(p))
@@ -52,18 +53,6 @@ def measured_peaks():
         except Exception:
             pass
     return out
-
-
-def ncu_traffic(kernel):
-    """dram bytes per launch of `kernel` from the newest committed ncu capture (profiles/*_traffic.json), or None"""
-    names = {"eval_paths": "eval_dp_kernel", "scatter": "scatter_kernel", "lev_match": "lev_match_kernel", "act_compact": "act_compact_kernel",
-             "pair_probe": "pair_probe_kernel", "emit": "emit_kernel", "vec_gemm_topk": "vec_gemm_topk_kernel", "vec_dist": "vec_dist_kernel"}
-    try:
-        import glob
-        f = sorted(glob.glob(os.path.join(ROOT, "profiles", "*_traffic.json")))[-1]
-        return float(json.load(open(f))["kernels"][names[kernel]]["dram_bytes_per_launch"])
-    except Exception:
-        return None
 
 
 class ClockSampler:
@@ -138,7 +127,7 @@ def workload_config(args, img):
                 "execute_hybrid(semanticRatio 0.5), keyword side ScoringStrategy::Detailed")
     return {"workload": txt, "mode": args.mode, "batch": args.batch, "docs": int(img.n_docs), "vocab": int(img.n_words),
             "l2": "working set (posting store, per-batch matrices" + (", 15.4 GB embedding matrix" if args.mode == "hybrid" else "") +
-                  ") exceeds the 126 MB L2; a different query batch every step"}
+                  ") exceeds the 50 MB L2; a different query batch every step"}
 
 
 # ------------------------------------------------------------------------------------------------ CPU arm
@@ -287,7 +276,7 @@ def run_parity(args, ix, img, emb, batches, vecs):
 # ------------------------------------------------------------------------------------------------ cfg 5: corpus-sharded vector stage
 def sharded_vector_stage(args, ix, rank, world, local_rank):
     """SURVEY §8(e) / cfg 5, vector side: the embedding matrix is partitioned by contiguous docid range, 12.5 M x 768 fp16 rows per
-    GPU (100 M at 8 GPUs).  Every rank scans its shard for the SAME 1024 queries (tcgen05 GEMM + fused top-100), the per-shard
+    GPU (100 M at 8 GPUs).  Every rank scans its shard for the SAME 1024 queries (wgmma GEMM + fused top-100), the per-shard
     top-100 lists are exchanged with one ncclAllGather issued by the library on its own stream and merged on the device
     (b200_nns_batch_sharded).  First a 1 M-row subsample is checked against the single-shard CPU oracle."""
     import torch
@@ -370,6 +359,7 @@ def main():
     ap.add_argument("--parity", type=int, default=0, help="queries of the parity check (0 = the whole batch)")
     ap.add_argument("--no-extras", action="store_true", help="skip the secondary vector-stage measurements")
     ap.add_argument("--shard-rows", type=int, default=12_500_000, help="embedding rows per GPU of the corpus-sharded stage (N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the result arrays of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -432,6 +422,8 @@ def main():
     if world > 1:
         dist.barrier()
     clocks = sampler.stop((t0, t0 + wall))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(res, args.dump_outputs)
     st_e2e = ix.stats()
     n_ok = int((res.status == 0).sum())
     # second timed region, software pipeline off (one lane): kernels of different lanes no longer overlap, so the CUDA-event
@@ -477,16 +469,16 @@ def main():
             flops = 2.0 * args.batch * float(img.n_docs) * DIM
             ach = flops / (per_launch_ms * 1e-3) / 1e12 if per_launch_ms > 0 else 0.0
             return {"bound": "tensor", "kernel": name, "achieved": ach, "peak": peaks["tensor"][0], "peak_source": peaks["tensor"][1], "unit": "TFLOP/s",
-                    "frac": ach / peaks["tensor"][0], "traffic": ncu_traffic(name), "launches": int(d["count"]), "avg_launch_ms": per_launch_ms,
+                    "frac": ach / peaks["tensor"][0], "launches": int(d["count"]), "avg_launch_ms": per_launch_ms,
                     "algorithmic_flops_per_launch": flops, "algorithmic_bytes_per_launch": d["bytes"] / d["count"]}
         ach = (d["bytes"] / d["count"]) / (per_launch_ms * 1e-3) / 1e9 if per_launch_ms > 0 else 0.0
         return {"bound": "hbm", "kernel": name, "achieved": ach, "peak": peaks["hbm"][0], "peak_source": peaks["hbm"][1], "unit": "GB/s",
-                "frac": ach / peaks["hbm"][0], "traffic": ncu_traffic(name), "launches": int(d["count"]), "avg_launch_ms": per_launch_ms,
+                "frac": ach / peaks["hbm"][0], "launches": int(d["count"]), "avg_launch_ms": per_launch_ms,
                 "algorithmic_bytes_per_launch": d["bytes"] / d["count"]}
 
     roofline = roof(dom)
     # a "launch" of the keyword kinds is the group of kernels of that kind in one device step, timed by one pair of CUDA events on the
-    # lane's stream (eval_paths = eval_dp_kernel of every shared-memory class + walk_kernel); `traffic` is ncu's DRAM bytes per such group
+    # lane's stream (eval_paths = eval_dp_kernel of every shared-memory class + walk_kernel)
     roofline["launch_unit"] = "one device step's kernels of this kind (eval_paths: eval_dp_kernel x classes + walk_kernel)"
     roofline["kernel_time_share"] = {k: round(v["ms"] / tot_ms, 4) for k, v in kern.items()}
     roofline["all_kernels"] = {k: {"frac": round(roof(k)["frac"], 4), "unit": roof(k)["unit"], "achieved": round(roof(k)["achieved"], 1),
@@ -545,6 +537,18 @@ def main():
     print(json.dumps(out), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+RESULT_ARRAYS = ("documents_ids", "n_hits", "n_scores", "score_kind", "score_rank", "score_max", "score_sim", "n_candidates",
+                 "semantic_hit_count", "status", "degraded", "used_negative_operator")
+
+
+def dump_outputs(res, out_dir):
+    """the SearchResult arrays a caller of the timed path receives, as float64 (every integer field is exact there): with the same
+    arguments the inputs are the same seeded corpus and batches, so two builds can be compared array by array"""
+    os.makedirs(out_dir, exist_ok=True)
+    for name in RESULT_ARRAYS:
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(getattr(res, name), np.float64))
 
 
 def extras(args, ix, img, emb, batches, out, peaks):

@@ -10,7 +10,7 @@
  *   crates/milli/src/update/new/extract/searchable/extract_word_pair_proximity_docids.rs:470-560
  *   crates/milli/src/update/new/extract/searchable/tokenize_document.rs:13-14,128-150
  *   crates/milli/src/update/new/word_fst_builder.rs:71-131 (prefix dbs)
- * Both the CPU oracle and the B200 library are fed from these byte images, exactly as a
+ * Both the CPU oracle and the CUDA library are fed from these byte images, exactly as a
  * deployment would feed them from the LMDB environment.
  */
 #ifndef B200_INDEXGEN_H

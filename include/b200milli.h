@@ -1,4 +1,4 @@
-/* b200milli — B200-native (sm_100a) implementation of milli's query-time scoring path.
+/* b200milli — H100-native (sm_90a) implementation of milli's query-time scoring path.
  *
  * C ABI of the drop-in boundary (SURVEY.md §8(b)).  The reference has no FFI for this path; its
  * seams are Rust-internal.  Each entry point names the reference interface a Rust shim would

@@ -1,4 +1,4 @@
-"""meilisearch_b200 — B200-native (sm_100a) implementation of milli's query-time scoring path.
+"""meilisearch_b200 — H100-native (sm_90a) implementation of milli's query-time scoring path.
 
 Python host-side mirror of the reference interface for this path (crates/milli/src/search/mod.rs:58-86,280-415,526-535):
 `Index` (the staged, HBM-resident copy of what `milli::Index` exposes to search), the `Search` builder with
@@ -65,7 +65,7 @@ KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "e
 
 
 def build_library(force=False):
-    """Compile the CUDA extension in-tree for sm_100a (works without a GPU)."""
+    """Compile the CUDA extension in-tree for sm_90a (works without a GPU)."""
     csrc = os.path.join(_HERE, "csrc")
     srcs = [os.path.join(csrc, f) for f in os.listdir(csrc) if f.endswith((".cu", ".cpp", ".h"))] + [os.path.join(_HERE, "..", "include", "b200milli.h")]
     if force or not os.path.exists(LIB_PATH) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in srcs):

@@ -408,7 +408,7 @@ struct Engine {
         }
         vstats = b200_stats{};
     }
-    int sm_count = 148;
+    int sm_count = 132;
     // pools
     uint8_t *arena = nullptr;
     size_t arena_bytes = 0;

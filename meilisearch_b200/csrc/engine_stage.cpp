@@ -174,8 +174,8 @@ int Engine::stage_finish() {
         const char *v = getenv(name);
         return v ? (size_t)atoll(v) << 20 : dflt;
     };
-    // sized for 180 GB of HBM: a sixth of what is free each (capped; two handles can coexist), the rest stays for the embeddings staged afterwards and
-    // the row lookup tables; a 10 M-document index at batch 256 needs ~ 30 GB of scratch for its widest rule step
+    // a sixth of what is free each (capped; two handles can coexist): about 13 GB each on an 80 GB card, and the rest stays for the
+    // embeddings staged afterwards (15.4 GB at 10 M x 768 fp16) and the row lookup tables
     arena_bytes = env_mb("B200_ARENA_MB", std::min<size_t>(free_b / 6, (size_t)32 << 30));
     scratch_bytes = env_mb("B200_SCRATCH_MB", std::min<size_t>(free_b / 6, (size_t)40 << 30));
     CU(cudaMalloc((void **)&arena, arena_bytes), "alloc arena");
@@ -367,7 +367,7 @@ int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t l
         CU(cudaMemcpyAsync(d_cand.p, cand, n_cand_words * 8, cudaMemcpyHostToDevice, vt.stream), "H2D candidates");
         d_c = d_cand.p;
     }
-    // ---- batched path: tcgen05 GEMM with the top-k fused into its epilogue (vec_gemm.cu)
+    // ---- batched path: wgmma GEMM with the top-k fused into its epilogue (vec_gemm.cu)
     {
         const char *force = getenv("B200_VEC_GEMM");
         bool want = force ? atoi(force) != 0 : n_q >= 16;
@@ -380,14 +380,15 @@ int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t l
             const uint32_t tiles_per_pass = vec_sms;  // query tiles resident in one launch
             std::vector<uint32_t> h_ids, h_n;
             std::vector<float> h_dist;
-            for (uint32_t q0 = 0; q0 < n_q; q0 += tiles_per_pass * 128) {
-                uint32_t nq = std::min<uint32_t>(n_q - q0, tiles_per_pass * 128);
-                uint32_t n_qtiles = (nq + 127) / 128, n_pad = n_qtiles * 128;
+            constexpr uint32_t TQ = VEC_GEMM_QTILE;  // queries per tile of the kernel
+            for (uint32_t q0 = 0; q0 < n_q; q0 += tiles_per_pass * TQ) {
+                uint32_t nq = std::min<uint32_t>(n_q - q0, tiles_per_pass * TQ);
+                uint32_t n_qtiles = (nq + TQ - 1) / TQ, n_pad = n_qtiles * TQ;
                 uint64_t n_row_tiles = (N + 63) / 64;
                 uint32_t n_groups = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)vec_sms / n_qtiles, n_row_tiles));
                 CU(d_vq.reserve((size_t)nq * d + n_pad), "alloc queries");
                 CU(d_vq16.reserve((size_t)n_pad * d), "alloc fp16 queries");
-                CU(d_vruns.reserve((size_t)n_qtiles * n_groups * 128 * VEC_GEMM_CAND_CAP + (size_t)n_pad * n_groups), "alloc candidate runs");
+                CU(d_vruns.reserve((size_t)n_qtiles * n_groups * TQ * VEC_GEMM_CAND_CAP + (size_t)n_pad * n_groups), "alloc candidate runs");
                 CU(d_vpartial.reserve((size_t)n_pad * n_groups * VEC_GEMM_KMAX), "alloc partial top-k");
                 CU(d_vsel_dist.reserve((size_t)n_pad * limit), "alloc selection");
                 CU(d_vsel_ids.reserve((size_t)n_pad * limit), "alloc selection");
@@ -399,7 +400,7 @@ int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t l
                 vstats.kernel_launches++;
                 size_t m0 = vt.mark();
                 CU(launch_vec_gemm_topk(vt.stream, vec_sms, dix.emb, dix.emb_inv_norm, dix.emb_docids, N, d, d_vq16.p, d_qinv, n_qtiles, n_groups,
-                                        d_c, n_cand_words, limit, d_vruns.p + (size_t)n_qtiles * n_groups * 128 * VEC_GEMM_CAND_CAP, d_vruns.p, d_vpartial.p, d_vsel_ids.p, d_vsel_dist.p, d_vsel_n.p, nq),
+                                        d_c, n_cand_words, limit, d_vruns.p + (size_t)n_qtiles * n_groups * TQ * VEC_GEMM_CAND_CAP, d_vruns.p, d_vpartial.p, d_vsel_ids.p, d_vsel_dist.p, d_vsel_n.p, nq),
                    "vec_gemm_topk");
                 if (sharded && sc.world > 1) {
                     // one all-gather of the per-shard top-k (ids, distances, counts) on the vector stream, then the merge: the lists

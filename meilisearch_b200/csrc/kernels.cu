@@ -1,4 +1,4 @@
-// CUDA kernels for sm_100a.  HBM/L2-bound integer work: 128-bit coalesced loads where rows are streamed,
+// CUDA kernels for sm_90a.  HBM/L2-bound integer work: 128-bit coalesced loads where rows are streamed,
 // warp shuffles/ballots for reductions and ordered compaction, no tensor cores (DESIGN.md §4).
 //
 //   lev_match_kernel / lev_finalize_kernel   term derivation: Levenshtein(<=2, transposition) x dictionary

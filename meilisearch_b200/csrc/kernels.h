@@ -44,16 +44,18 @@ cudaError_t launch_emb_norm_f16(cudaStream_t s, const void *rows_fp16, float *in
 cudaError_t launch_shard_merge(cudaStream_t s, const uint32_t *g_ids, const float *g_dist, const uint32_t *g_n, uint32_t world, uint32_t n_q,
                                uint32_t k, uint32_t *out_ids, float *out_dist, uint32_t *out_n);
 
-// ---- vec_gemm.cu: batched vector stage on tcgen05 (queries x matrix^T with the top-k fused into the epilogue)
+// ---- vec_gemm.cu: batched vector stage on wgmma (queries x matrix^T with the top-k fused into the epilogue)
+#define VEC_GEMM_QTILE 64
 #define VEC_GEMM_CAND_CAP 256
 #define VEC_GEMM_KMAX 128
 bool vec_gemm_supported(uint32_t d, uint32_t limit);
-size_t vec_gemm_smem_bytes(uint32_t d, bool ts);
+size_t vec_gemm_smem_bytes(uint32_t d);
 cudaError_t launch_vec_prep_queries(cudaStream_t s, const float *q, uint32_t n_q, uint32_t n_pad, uint32_t d, void *out_fp16, float *inv);
-// runs: n_qtiles*n_groups*128*VEC_GEMM_CAND_CAP u64 scratch; partial: n_qtiles*128*n_groups*VEC_GEMM_KMAX u64
+// query tiles of VEC_GEMM_QTILE rows; runs: n_qtiles*n_groups*VEC_GEMM_QTILE*VEC_GEMM_CAND_CAP u64 scratch;
+// partial: n_qtiles*VEC_GEMM_QTILE*n_groups*VEC_GEMM_KMAX u64
 cudaError_t launch_vec_gemm_topk(cudaStream_t s, uint32_t sm_count, const void *mat_fp16, const float *inv_norm, const uint32_t *docids,
                                  uint64_t n_rows, uint32_t d, const void *q_fp16, const float *q_inv_norm, uint32_t n_qtiles, uint32_t n_groups,
-                                 const unsigned long long *cand, uint64_t n_cand_words, uint32_t k, unsigned long long *gthr /* n_qtiles*128*n_groups u64 */,
+                                 const unsigned long long *cand, uint64_t n_cand_words, uint32_t k, unsigned long long *gthr /* n_qtiles*VEC_GEMM_QTILE*n_groups u64 */,
                                  unsigned long long *runs,
                                  unsigned long long *partial, uint32_t *out_ids, float *out_dist, uint32_t *out_n, uint32_t n_q);
 }  // namespace b200

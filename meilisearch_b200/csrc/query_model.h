@@ -1,5 +1,5 @@
 // Host-side query model of the engine: terms, term subsets, query graph, ranking-rule graph.
-// B200-native restatement (word ids are dictionary ranks, derivations arrive from the device):
+// GPU-native restatement (word ids are dictionary ranks, derivations arrive from the device):
 //   crates/milli/src/search/new/query_term/{mod.rs,ntypo_subset.rs,parse_query.rs,compute_derivations.rs:170-253}
 //   crates/milli/src/search/new/query_graph.rs
 //   crates/milli/src/search/new/ranking_rule_graph/{build.rs,mod.rs} and the six rule directories

@@ -1,20 +1,22 @@
-// Batched vector stage on the 5th-gen tensor cores: distances of a tile of 128 query vectors against the staged fp16
-// embedding matrix, with the exact top-k selection fused into the epilogue (the distance matrix never exists in HBM).
+// Batched vector stage on the Hopper tensor cores: distances of a tile of 64 query vectors against the staged fp16 embedding
+// matrix, with the exact top-k selection fused into the epilogue (the distance matrix never exists in HBM).
 //
 // Replaces, for a batch of semantic / hybrid queries, B calls of VectorStore::nns_by_vector
 // (crates/milli/src/vector/store.rs:638-645, reached from VectorSort::fill_buffer, ranking_rules/vector_sort.rs:58-78)
 // with one exhaustive scan: distance = (1 - cos)/2 (arroy/hannoy `Cosine`), ascending, ties by docid.
 //
 // Per CTA (one per SM, 256 threads):
-//   warp 0   TMA producer: the query tile [128 x d] once (A operand, resident: d/64 blocks of 16 KB, 128B-swizzled, K-major),
-//            then matrix row tiles [64 rows x 64 halfs] through a 4-stage ring (B operand)
-//   warp 1   one thread issues tcgen05.mma.cta_group::1.kind::f16 (M=128 queries, N=64 rows, K=16) into one of four TMEM accumulators
-//   warp 2   TMEM allocation (256 columns)
-//   warp 3   stages each row tile's docids (filtered rows marked) and inverse norms in shared memory, one tile ahead
-//   warps 4-7  epilogue: lane = query; tcgen05.ld of 64 fp32 dots, distance, compare with the query's running threshold, append
-//            survivors to the query's candidate run in L2-resident scratch; a warp-cooperative bitonic sort compacts a run to its
-//            k best whenever it fills up, which tightens the threshold.
+//   warp 0     TMA producer: the query tile [64 x d] once (A operand, resident: d/64 blocks of 8 KB, 128B-swizzled, K-major),
+//              then matrix row tiles [64 rows x 64 halfs] through an 8-stage ring (B operand)
+//   warp 1     stages each row tile's docids (filtered rows marked) and inverse norms in shared memory, one tile ahead
+//   warps 2-3  epilogue: lane = query; reads the tile's 64 fp32 dots from the accumulator staging buffer, distance, compare with
+//              the query's running threshold, append survivors to the query's candidate run in L2-resident scratch; a
+//              warp-cooperative bitonic sort compacts a run to its k best whenever it fills up, which tightens the threshold.
+//   warps 4-7  one warpgroup issues wgmma.mma_async m64n64k16 (f16 in, f32 accumulators in registers) over the k-blocks of a row
+//              tile, then writes the accumulators to one of two staging buffers in shared memory for the epilogue
 // CTA c serves query tile c % n_qtiles and the c / n_qtiles-th slice of the row tiles; vec_merge_kernel merges the slices.
+// The query tile is 64 rows (one warpgroup's M) so that a 768-wide tile (96 KB), the matrix ring and the staging buffers fit in
+// the 227 KB of shared memory a block may use.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -22,7 +24,6 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
-#include <vector>
 
 #include "kernels.h"
 
@@ -30,18 +31,20 @@ namespace b200 {
 
 namespace {
 
-constexpr int GM = 128;        // queries per tile (UMMA M)
-constexpr int GN = 64;         // matrix rows per tile (UMMA N)
-constexpr int GK = 64;         // halfs per k-block = one 128-byte swizzle span
-constexpr int STAGES = 4;      // B ring when the query tile occupies shared memory (SS form)
-constexpr int STAGES_TS = 24;  // B ring when the query tile lives in TMEM (TS form): 192 KB in flight per SM
-constexpr int A_COLS = 384;    // TMEM columns of a 128 x 768 fp16 query tile (2 halfs per 32-bit column)
-constexpr int ACC_BUFS = 4;    // TMEM accumulators of GN columns each
-constexpr int META_BUFS = 2;   // row metadata (docid, inverse norm) staged per tile by warp 3
-constexpr int A_BLOCK = GM * GK * 2;  // 16 KB
-constexpr int B_BLOCK = GN * GK * 2;  // 8 KB
+constexpr int GM = VEC_GEMM_QTILE;  // queries per tile (wgmma M of one warpgroup)
+constexpr int GN = 64;              // matrix rows per tile (wgmma N)
+constexpr int GK = 64;              // halfs per k-block = one 128-byte swizzle span
+constexpr int STAGES = 8;           // B ring depth
+constexpr int NACC = 2;             // accumulator staging buffers
+constexpr int ACC_LD = GM + 4;      // floats per staged column: the fragment stores and the per-query loads are bank-conflict free
+constexpr int META_BUFS = 2;        // row metadata (docid, inverse norm) staged per tile by warp 1
+constexpr int EPI_WARPS = GM / 32;  // epilogue warps, one query per lane
+constexpr int A_BLOCK = GM * GK * 2;        // 8 KB
+constexpr int B_BLOCK = GN * GK * 2;        // 8 KB
+constexpr int ACC_BYTES = GN * ACC_LD * 4;  // 17 KB
 constexpr int CAND_CAP = VEC_GEMM_CAND_CAP;
 constexpr int KMAX = VEC_GEMM_KMAX;
+static_assert(GM % 32 == 0 && 2 + EPI_WARPS <= 4, "epilogue warps must fit between warp 1 and the MMA warpgroup");
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -54,8 +57,8 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// BACKOFF > 0: sleep that many nanoseconds after a failed poll — the single-thread roles share their scheduler with an epilogue
-// warp, and a tight polling loop takes half of its issue slots
+// BACKOFF > 0: sleep that many nanoseconds after a failed poll — the single-thread roles share their scheduler with other warps,
+// and a tight polling loop takes their issue slots
 template <int BACKOFF = 0>
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     uint32_t addr = smem_u32(bar);
@@ -74,85 +77,53 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         if (++spins > (1ull << 26)) __trap();  // a lost arrival must not hang the device
     }
 }
-template <int BACKOFF = 0>
-__device__ __forceinline__ void mbar_wait_t(uint64_t *bar, uint32_t parity, unsigned long long &acc, bool on) {
-    if (!on) {
-        mbar_wait<BACKOFF>(bar, parity);
-        return;
-    }
-    long long t0 = clock64();
-    mbar_wait<BACKOFF>(bar, parity);
-    acc += (unsigned long long)(clock64() - t0);
-}
 __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, uint64_t *bar, int32_t c0, int32_t c1) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
                  "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
                  : "memory");
 }
-// one lane of a converged warp (the role loops run warp-convergent so that descriptors and ring counters live in uniform
-// registers; only the issuing instructions are predicated on the elected lane — a loop under `if (lane == 0)` pays a register ->
-// uniform-register move for every operand of every tcgen05.mma / TMA instruction)
+// one lane of a converged warp (the producer loop runs warp-convergent; only the issuing instructions are predicated)
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred != 0;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// K-major, 128-byte swizzle: 8-row groups are 1024 B apart (SBO); LBO is unused for swizzled K-major operands.
-// Field layout: cute/arch/mma_sm100_desc.hpp (start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout [61,64) = 2).
+// wgmma shared-memory descriptor, K-major with the 128-byte swizzle: 8-row groups are 1024 B apart (stride byte offset), the
+// leading byte offset is unused for swizzled K-major operands.  Fields: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
+// layout [62,64) = 1 (128B swizzle).  A K=16 step inside the swizzle span advances the start address by 32 B.
 __device__ __forceinline__ uint64_t make_sdesc(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3ffff) >> 4);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// kind::f16 instruction descriptor: D=f32 (bits[4,6)=1), A=B=f16 (0), both K-major, N>>3 at [17,23), M>>4 at [24,29).
-constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(GN >> 3) << 17) | ((uint32_t)(GM >> 4) << 24);
-
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator accesses across the asynchronous MMA
+__device__ __forceinline__ void acc_fence(float (&d)[32]) {
+#pragma unroll
+    for (int i = 0; i < 32; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(IDESC), "r"(accumulate)
-        : "memory");
-}
-// A operand from tensor memory (lane = row, 32-bit column = two consecutive K elements), B from shared memory
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(bdesc), "r"(IDESC), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t *r) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]),
-        "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]),
-        "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t *r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-          "=r"(r[31])
-        : "r"(taddr)
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+          "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+          "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
 
@@ -232,34 +203,21 @@ __device__ __forceinline__ float reject_bound(unsigned long long thr, float qn) 
 
 }  // namespace
 
-// TS = true: the query tile is written to tensor memory once (tcgen05.st by the epilogue warps) and read by the MMA from there,
-// which leaves all of shared memory to the matrix ring (24 stages instead of 4: the stream is latency x bandwidth bound).
-template <bool TS>
 __global__ void __launch_bounds__(256, 1)
-    vec_gemm_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_m, const __half *__restrict__ q_fp16,
-                         uint32_t d, uint64_t n_rows, uint32_t kblocks,
+    vec_gemm_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_m, uint64_t n_rows, uint32_t kblocks,
                          uint32_t n_qtiles, uint32_t n_groups, const float *__restrict__ inv_norm, const uint32_t *__restrict__ docids,
                          const float *__restrict__ q_inv_norm, const unsigned long long *__restrict__ cand, uint64_t n_cand_words, uint32_t kk,
-                         unsigned long long *__restrict__ gthr /* [n_qtiles*128][n_groups], init ~0: each slice's ceil(k/n_groups)-th best key so far */,
-                         unsigned long long *__restrict__ runs /* [cta][128][CAND_CAP] */,
-                         unsigned long long *__restrict__ partial /* [n_qtiles*128][n_groups][KMAX] */,
-                         unsigned long long *__restrict__ dbg /* optional [cta][8] cycle counters, see B200_VEC_DEBUG */, uint32_t dbg_mode) {
+                         unsigned long long *__restrict__ gthr /* [n_qtiles*GM][n_groups], init ~0: each slice's ceil(k/n_groups)-th best key so far */,
+                         unsigned long long *__restrict__ runs /* [cta][GM][CAND_CAP] */,
+                         unsigned long long *__restrict__ partial /* [n_qtiles*GM][n_groups][KMAX] */) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    constexpr int NST = TS ? STAGES_TS : STAGES;      // B ring depth
-    constexpr int NACC = 2;                           // tile buffers in TMEM
-    // SS: every tile accumulates into KS = 2 accumulators (even / odd k-blocks) that the epilogue adds: consecutive MMAs into one
-    // accumulator serialise on its latency (~100 cycles at N = 64), two independent chains keep the tensor pipe busy
-    constexpr int KS = TS ? 1 : 2;
-    const uint32_t ks = (KS == 2 && kblocks >= 2) ? 2u : 1u;  // a single k-block leaves the odd accumulator unused
-    constexpr uint32_t ACC_COL0 = TS ? A_COLS : 0;    // first accumulator column
-    constexpr uint32_t TMEM_COLS = TS ? 512 : ACC_BUFS * GN;
     uint8_t *sA = smem;
-    uint8_t *sB = TS ? smem : smem + (size_t)kblocks * A_BLOCK;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sB + NST * B_BLOCK);
-    uint64_t *a_full = bars, *b_full = bars + 1, *b_empty = b_full + NST, *acc_full = b_empty + NST, *acc_empty = acc_full + NACC;
+    uint8_t *sB = sA + (size_t)kblocks * A_BLOCK;
+    float *sAcc = reinterpret_cast<float *>(sB + STAGES * B_BLOCK);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sAcc + NACC * (ACC_BYTES / 4));
+    uint64_t *a_full = bars, *b_full = bars + 1, *b_empty = b_full + STAGES, *acc_full = b_empty + STAGES, *acc_empty = acc_full + NACC;
     uint64_t *meta_full = acc_empty + NACC, *meta_empty = meta_full + META_BUFS;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(meta_empty + META_BUFS);
     // row metadata ring: static shared memory, so that the epilogue reads it with (vectorisable) LDS instead of generic loads
     __shared__ __align__(16) uint32_t s_doc[META_BUFS * GN];
     __shared__ __align__(16) float s_scale[META_BUFS * GN];
@@ -271,126 +229,44 @@ __global__ void __launch_bounds__(256, 1)
     const uint64_t tile_lo = n_tiles * group / n_groups, tile_hi = n_tiles * (group + 1) / n_groups;
 
     if (threadIdx.x == 0) {
-        mbar_init(a_full, TS ? 4 : 1);  // TS: one arrival per epilogue warp once its 32 query rows are in TMEM
-        for (int s = 0; s < NST; s++) {
+        mbar_init(a_full, 1);
+        for (int s = 0; s < STAGES; s++) {
             mbar_init(b_full + s, 1);
             mbar_init(b_empty + s, 1);
         }
         for (int b = 0; b < NACC; b++) {
-            mbar_init(acc_full + b, 1);
-            mbar_init(acc_empty + b, 4);
+            mbar_init(acc_full + b, 128);             // every thread of the MMA warpgroup, after its fragment stores
+            mbar_init(acc_empty + b, EPI_WARPS * 32); // every epilogue thread, after its last read of the buffer
         }
         for (int b = 0; b < META_BUFS; b++) {
             mbar_init(meta_full + b, 1);
-            mbar_init(meta_empty + b, 4);
+            mbar_init(meta_empty + b, EPI_WARPS);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == 0) {
         const bool leader = elect_one();
-        if (!TS && leader) {
+        if (leader) {
             mbar_expect_tx(a_full, kblocks * A_BLOCK);
             for (uint32_t kb = 0; kb < kblocks; kb++) tma_load_2d(sA + (size_t)kb * A_BLOCK, &tmap_q, a_full, (int32_t)(kb * GK), (int32_t)(qtile * GM));
         }
         uint32_t s = 0, ph = 0;
-        unsigned long long w_prod = 0;
         for (uint64_t t = tile_lo; t < tile_hi; t++)
             for (uint32_t kb = 0; kb < kblocks; kb++) {
-                mbar_wait_t<128>(b_empty + s, ph ^ 1, w_prod, false);
+                mbar_wait<128>(b_empty + s, ph ^ 1);
                 if (leader) {
                     mbar_expect_tx(b_full + s, B_BLOCK);
                     tma_load_2d(sB + (size_t)s * B_BLOCK, &tmap_m, b_full + s, (int32_t)(kb * GK), (int32_t)(t * GN));
                 }
                 __syncwarp();
-                if (++s == (uint32_t)NST) {
+                if (++s == (uint32_t)STAGES) {
                     s = 0;
                     ph ^= 1;
                 }
             }
-    } else if (warp == 1 || warp == 2) {
-        // Two MMA issuers (one thread each), alternating tiles: at N = 64 a K-block is only 4 x 32 cycles of tensor work, less than
-        // what one thread needs to wait for the stage, build the descriptors and issue — one issuer alone leaves the tensor pipe idle
-        // two thirds of the time.  Issuer p owns tile buffer p and the ring stages of the tiles of its parity.
-        {
-            const bool leader = elect_one();
-            const uint32_t par = warp - 1;
-            // mbarrier parity waits are only unambiguous one phase ahead: with two issuers a ring stage must always come back to
-            // the issuer that consumed its previous phase, i.e. the ring must hold a whole number of tile PAIRS
-            const bool dual = (uint32_t)NST % (2 * kblocks) == 0;
-            const uint32_t step = dual ? 2 : 1;
-            if (par == 0 || dual) {
-            mbar_wait(a_full, 0);
-            tc_fence_after();
-            uint32_t s = 0, ph = 0;  // ring position of this issuer's next stage
-            if (par) {
-                s += kblocks;
-                while (s >= (uint32_t)NST) {
-                    s -= NST;
-                    ph ^= 1;
-                }
-            }
-            const uint64_t bd0 = make_sdesc(smem_u32(sB));
-            const uint64_t ad0 = TS ? 0ull : make_sdesc(smem_u32(sA));
-            unsigned long long w_acc = 0, w_b = 0;
-            const long long t_mma0 = clock64();
-            uint32_t n = par;
-            for (uint64_t t = tile_lo + par; t < tile_hi; t += step, n += step) {
-                const uint32_t buf = n & 1, aph = (n >> 1) & 1;
-                mbar_wait_t<32>(acc_empty + buf, aph ^ 1, w_acc, dbg != nullptr);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + ACC_COL0 + buf * (KS * GN);
-                for (uint32_t kb = 0; kb < kblocks; kb++) {
-                    mbar_wait_t<32>(b_full + s, ph, w_b, dbg != nullptr);
-                    tc_fence_after();
-                    const uint64_t bd = bd0 + (uint64_t)s * (B_BLOCK >> 4);
-                    if (TS) {
-#pragma unroll
-                        for (uint32_t k = 0; k < GK / 16; k++)  // 8 TMEM columns (16 halfs) and 32 B of the B row per K=16 step
-                            if (leader) umma_ts(tmem_d, tmem_base + kb * (GK / 2) + k * 8, bd + 2 * k, (kb | k) != 0);
-                    } else {
-                        const uint64_t ad = ad0 + (uint64_t)kb * (A_BLOCK >> 4);
-                        const uint32_t acc = tmem_d + (kb & (ks - 1)) * GN;  // even / odd k-blocks: two accumulation chains
-#pragma unroll
-                        for (uint32_t k = 0; k < GK / 16; k++)
-                            if (leader) umma(acc, ad + 2 * k, bd + 2 * k, (kb >= ks) || k != 0);  // +32 B per K=16 step
-                    }
-                    if (leader) tc_commit(b_empty + s);
-                    __syncwarp();
-                    if (++s == (uint32_t)NST) {
-                        s = 0;
-                        ph ^= 1;
-                    }
-                }
-                if (leader) tc_commit(acc_full + buf);
-                __syncwarp();
-                if (dual) {
-                    s += kblocks;  // the other issuer's tile
-                    while (s >= (uint32_t)NST) {
-                        s -= NST;
-                        ph ^= 1;
-                    }
-                }
-            }
-            if (dbg && par == 0 && leader) {
-                dbg[blockIdx.x * 8 + 3] = (unsigned long long)(clock64() - t_mma0);
-                if (dbg_mode == 2) {
-                    dbg[blockIdx.x * 8 + 1] = w_acc;
-                    dbg[blockIdx.x * 8 + 2] = w_b;
-                }
-            }
-            }
-        }
-    } else if (warp == 3) {
+    } else if (warp == 1) {
         uint32_t n = 0;
         for (uint64_t t = tile_lo; t < tile_hi; t++, n++) {
             const uint32_t mb = n % META_BUFS, mph = (n / META_BUFS) & 1;
@@ -413,30 +289,61 @@ __global__ void __launch_bounds__(256, 1)
             if (lane == 0) mbar_arrive(meta_full + mb);
         }
     } else if (warp >= 4) {
-        const uint32_t w = warp - 4;  // == warp % 4: the TMEM lane quarter this warp may read
-        const uint32_t qrow = qtile * GM + w * 32 + lane;
-        const float qn = q_inv_norm[qrow];
-        unsigned long long *my_run = runs + ((size_t)blockIdx.x * GM + w * 32 + lane) * CAND_CAP;
-        unsigned long long *warp_runs = runs + ((size_t)blockIdx.x * GM + w * 32) * CAND_CAP;
-        if (TS) {  // this thread's query row -> TMEM lane w*32+lane, columns [0, d/2)
-            const uint32_t *src = reinterpret_cast<const uint32_t *>(q_fp16 + (size_t)qrow * d);
-            for (uint32_t c0 = 0; c0 < d / 2; c0 += 32) {
-                uint32_t regs[32];
+        // MMA warpgroup: accumulators of a whole row tile in registers (32 fp32 per thread), one commit group per k-block; the ring
+        // stage of k-block kb is released once the group of kb + 1 is issued and that of kb has completed
+        const uint32_t wq = warp - 4, g = lane >> 2, q = lane & 3;
+        const uint64_t ad0 = make_sdesc(smem_u32(sA)), bd0 = make_sdesc(smem_u32(sB));
+        mbar_wait(a_full, 0);
+        uint32_t s = 0, ph = 0, n = 0;
+        for (uint64_t t = tile_lo; t < tile_hi; t++, n++) {
+            float acc[32];
 #pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    uint4 x = __ldg(reinterpret_cast<const uint4 *>(src + c0) + i);
-                    regs[4 * i] = x.x;
-                    regs[4 * i + 1] = x.y;
-                    regs[4 * i + 2] = x.z;
-                    regs[4 * i + 3] = x.w;
+            for (int i = 0; i < 32; i++) acc[i] = 0.f;
+            uint32_t prev = 0;
+            for (uint32_t kb = 0; kb < kblocks; kb++) {
+                mbar_wait(b_full + s, ph);
+                wgmma_fence();
+                acc_fence(acc);
+                const uint64_t ad = ad0 + (uint64_t)kb * (A_BLOCK >> 4), bd = bd0 + (uint64_t)s * (B_BLOCK >> 4);
+#pragma unroll
+                for (uint32_t k = 0; k < GK / 16; k++) wgmma_m64n64k16(acc, ad + 2 * k, bd + 2 * k, (kb | k) != 0);  // +32 B per K=16 step
+                wgmma_commit();
+                acc_fence(acc);
+                if (kb > 0) {
+                    wgmma_wait<1>();
+                    if (threadIdx.x == 128) mbar_arrive(b_empty + prev);
                 }
-                tmem_st32(tmem_base + ((w * 32u) << 16) + c0, regs);
+                prev = s;
+                if (++s == (uint32_t)STAGES) {
+                    s = 0;
+                    ph ^= 1;
+                }
             }
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(a_full);
+            wgmma_wait<0>();
+            acc_fence(acc);
+            if (threadIdx.x == 128) mbar_arrive(b_empty + prev);
+            // fragment -> staging buffer, column-major: element (query r, row c) at c * ACC_LD + r.  Thread (warp wq, lane) holds
+            // queries 16 wq + g and 16 wq + g + 8, rows 8 i + 2 q and 8 i + 2 q + 1 of every n8 block i.
+            const uint32_t buf = n & 1, aph = (n >> 1) & 1;
+            mbar_wait(acc_empty + buf, aph ^ 1);
+            float *dst = sAcc + buf * (ACC_BYTES / 4) + wq * 16 + g;
+#pragma unroll
+            for (int i = 0; i < GN / 8; i++) {
+                const uint32_t c = 8 * i + 2 * q;
+                dst[c * ACC_LD] = acc[4 * i];
+                dst[(c + 1) * ACC_LD] = acc[4 * i + 1];
+                dst[c * ACC_LD + 8] = acc[4 * i + 2];
+                dst[(c + 1) * ACC_LD + 8] = acc[4 * i + 3];
+            }
+            mbar_arrive(acc_full + buf);
         }
+    } else if (warp >= 2 && warp < 2 + EPI_WARPS) {
+        const uint32_t w = warp - 2;
+        const uint32_t qcol = w * 32 + lane;  // this lane's query inside the tile
+        const uint32_t qrow = qtile * GM + qcol;
+        const float qn = q_inv_norm[qrow];
+        unsigned long long *my_run = runs + ((size_t)blockIdx.x * GM + qcol) * CAND_CAP;
+        unsigned long long *warp_runs = runs + ((size_t)blockIdx.x * GM + w * 32) * CAND_CAP;
         uint32_t cnt = 0;
         unsigned long long thr = ~0ull;
         float tq = __int_as_float(0xff800000);  // -inf: nothing is rejected before a threshold exists
@@ -450,112 +357,66 @@ __global__ void __launch_bounds__(256, 1)
         for (int i = 0; i < KP_REG; i++) best[i] = ~0ull;
         unsigned long long published = ~0ull, best_kp = ~0ull;  // best_kp == best[kp - 1]
         uint32_t n = 0;
-        unsigned long long w_full = 0, w_meta = 0, w_cmp = 0, w_ld = 0, w_p1 = 0, w_p2 = 0, w_flag = 0, w_mine = 0;
-        const long long t_epi0 = clock64();
         for (uint64_t t = tile_lo; t < tile_hi; t++, n++) {
-            uint32_t buf = n % NACC, aph = (n / NACC) & 1;
-            mbar_wait_t(acc_full + buf, aph, w_full, dbg != nullptr);
-            tc_fence_after();
-            const long long t_l0 = dbg ? clock64() : 0;
-            uint32_t v[GN];
-            uint32_t taddr = tmem_base + ((w * 32u) << 16) + ACC_COL0 + buf * (KS * GN);
-            tmem_ld32(taddr, v);
-            tmem_ld32(taddr + 32, v + 32);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (ks == 2) {  // add the odd-k-block accumulator
+            const uint32_t buf = n % NACC, aph = (n / NACC) & 1;
+            mbar_wait(acc_full + buf, aph);
+            const float *col = sAcc + buf * (ACC_BYTES / 4) + qcol;
+            float v[GN];
 #pragma unroll
-                for (int h = 0; h < 2; h++) {
-                    uint32_t o[32];
-                    tmem_ld32(taddr + GN + h * 32, o);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int i = 0; i < 32; i++) v[h * 32 + i] = __float_as_uint(__uint_as_float(v[h * 32 + i]) + __uint_as_float(o[i]));
-                }
-            }
-            if (dbg) w_ld += (unsigned long long)(clock64() - t_l0);
+            for (int j = 0; j < GN; j++) v[j] = col[j * ACC_LD];
             const uint32_t mb = n % META_BUFS, mph = (n / META_BUFS) & 1;
-            mbar_wait_t(meta_full + mb, mph, w_meta, dbg != nullptr);
+            mbar_wait(meta_full + mb, mph);
             const uint32_t *tdoc = s_doc + mb * GN;
             const float *tscale = s_scale + mb * GN;
-            const long long t_p0 = dbg ? clock64() : 0;
             // pass 1, branch-free: which of the 64 rows can possibly beat this query's threshold ("dot x inverse row norm" space)
             uint32_t m_lo = 0, m_hi = 0;
 #pragma unroll
             for (int j = 0; j < 32; j++) {
-                m_lo |= (__uint_as_float(v[j]) * tscale[j] < tq) ? 0u : (1u << j);
-                m_hi |= (__uint_as_float(v[j + 32]) * tscale[j + 32] < tq) ? 0u : (1u << j);
+                m_lo |= (v[j] * tscale[j] < tq) ? 0u : (1u << j);
+                m_hi |= (v[j + 32] * tscale[j + 32] < tq) ? 0u : (1u << j);
             }
             uint32_t u_lo = __reduce_or_sync(0xffffffffu, m_lo), u_hi = __reduce_or_sync(0xffffffffu, m_hi);
-            const long long t_p1 = dbg ? clock64() : 0;
-            if (dbg) {
-                w_p1 += (unsigned long long)(t_p1 - t_p0);
-                w_flag += __popc(u_lo) + __popc(u_hi);
-                w_mine += __popc(m_lo) + __popc(m_hi);
-            }
             // pass 2: exact distance + append for the (rare) columns some lane flagged.  A compact loop over the set bits — the dot is
-            // re-read from tensor memory with a one-column tcgen05.ld — instead of 64 unrolled copies: the hot loop stays small
-            // enough for the instruction cache.
-            while (u_lo | u_hi) {  // warp-uniform; up to four flagged columns per round share one tcgen05.wait::ld
-                uint32_t js[4], vv[4], vo[4];
-                int nj = 0;
-#pragma unroll
-                for (int q = 0; q < 4; q++) {
-                    js[q] = 0;
-                    vv[q] = vo[q] = 0;
-                    if (u_lo | u_hi) {
-                        const uint32_t j = u_lo ? (uint32_t)__ffs(u_lo) - 1u : 32u + (uint32_t)__ffs(u_hi) - 1u;
-                        if (u_lo)
-                            u_lo &= u_lo - 1;
-                        else
-                            u_hi &= u_hi - 1;
-                        js[q] = j;
-                        nj = q + 1;
-                        asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(vv[q]) : "r"(taddr + j) : "memory");
-                        if (ks == 2) asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(vo[q]) : "r"(taddr + GN + j) : "memory");
+            // re-read from the staging buffer — instead of 64 unrolled copies: the hot loop stays small enough for the instruction cache.
+            while (u_lo | u_hi) {  // warp-uniform
+                const uint32_t j = u_lo ? (uint32_t)__ffs(u_lo) - 1u : 32u + (uint32_t)__ffs(u_hi) - 1u;
+                if (u_lo)
+                    u_lo &= u_lo - 1;
+                else
+                    u_hi &= u_hi - 1;
+                const uint32_t mm = j < 32 ? m_lo : m_hi;
+                if ((mm >> (j & 31)) & 1u) {
+                    const float dot = col[j * ACC_LD];
+                    const uint32_t doc = tdoc[j];
+                    const float pn = tscale[j] * qn;
+                    float dd = 0.f;
+                    if (pn > 0.f && isfinite(pn)) {
+                        float cs = dot * pn;
+                        cs = fminf(1.f, fmaxf(-1.f, cs));
+                        dd = (1.f - cs) * 0.5f;
                     }
-                }
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+                    const unsigned long long key = ((unsigned long long)__float_as_uint(dd) << 32) | doc;
+                    if (doc != 0xffffffffu && key < thr) {
+                        my_run[cnt++] = key;
+                        if (reg_best && key < best_kp) {  // improves this slice's kp best: sorted insertion, the largest falls off
+                            unsigned long long x = key;
 #pragma unroll
-                for (int q = 0; q < 4; q++) {
-                    const uint32_t j = js[q];
-                    const uint32_t mm = j < 32 ? m_lo : m_hi;
-                    if (q < nj && ((mm >> (j & 31)) & 1u)) {
-                        const float dot = ks == 2 ? __uint_as_float(vv[q]) + __uint_as_float(vo[q]) : __uint_as_float(vv[q]);
-                        const uint32_t doc = tdoc[j];
-                        const float pn = tscale[j] * qn;
-                        float dd = 0.f;
-                        if (pn > 0.f && isfinite(pn)) {
-                            float cs = dot * pn;
-                            cs = fminf(1.f, fmaxf(-1.f, cs));
-                            dd = (1.f - cs) * 0.5f;
-                        }
-                        const unsigned long long key = ((unsigned long long)__float_as_uint(dd) << 32) | doc;
-                        if (doc != 0xffffffffu && key < thr) {
-                            my_run[cnt++] = key;
-                            if (reg_best && key < best_kp) {  // improves this slice's kp best: sorted insertion, the largest falls off
-                                unsigned long long x = key;
-#pragma unroll
-                                for (int i = 0; i < KP_REG; i++) {
-                                    const unsigned long long lo = x < best[i] ? x : best[i], hi = x < best[i] ? best[i] : x;
-                                    best[i] = lo;
-                                    x = hi;
-                                }
-                                best_kp = best[0];
-#pragma unroll
-                                for (int i = 1; i < KP_REG; i++) best_kp = (uint32_t)i < kp ? best[i] : best_kp;
+                            for (int i = 0; i < KP_REG; i++) {
+                                const unsigned long long lo = x < best[i] ? x : best[i], hi = x < best[i] ? best[i] : x;
+                                best[i] = lo;
+                                x = hi;
                             }
+                            best_kp = best[0];
+#pragma unroll
+                            for (int i = 1; i < KP_REG; i++) best_kp = (uint32_t)i < kp ? best[i] : best_kp;
                         }
                     }
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(acc_empty + buf);
+            mbar_arrive(acc_empty + buf);
             __syncwarp();
             if (lane == 0) mbar_arrive(meta_empty + mb);
-            if (dbg) w_p2 += (unsigned long long)(clock64() - t_p1);
             bool changed = false;
-            const long long t_c0 = dbg ? clock64() : 0;
             // compaction: when a run is nearly full — and once right after the first tile, so that every slice publishes an early
             // bound (see below) instead of appending everything for three tiles
             uint32_t need = __ballot_sync(0xffffffffu, cnt > (uint32_t)(CAND_CAP - GN) || (!reg_best && n == 0 && cnt >= kp));
@@ -596,18 +457,6 @@ __global__ void __launch_bounds__(256, 1)
                 }
             }
             if (changed) tq = reject_bound(thr, qn);
-            if (dbg) w_cmp += (unsigned long long)(clock64() - t_c0);
-        }
-        if (dbg && w == 0 && lane == 0) {
-            dbg[blockIdx.x * 8 + 4] = w_flag;
-            dbg[blockIdx.x * 8 + 5] = w_mine;
-            dbg[blockIdx.x * 8 + 6] = w_cmp;
-            dbg[blockIdx.x * 8 + 7] = (unsigned long long)(clock64() - t_epi0);
-            dbg[blockIdx.x * 8 + 0] = w_ld;
-            if (dbg_mode != 2) {
-                dbg[blockIdx.x * 8 + 1] = w_p1;
-                dbg[blockIdx.x * 8 + 2] = w_p2;
-            }
         }
         // final: every lane's run sorted, its kk best written to this (query, group) slot
         __syncwarp();
@@ -629,12 +478,7 @@ __global__ void __launch_bounds__(256, 1)
             }
         }
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    }
 }
 
 // fp32 queries -> fp16 padded tile rows + inverse norms (one warp per query; rows >= n_q are zero)
@@ -717,8 +561,9 @@ bool make_map(CUtensorMap *m, const void *base, uint64_t rows, uint32_t d, uint3
 }
 }  // namespace
 
-size_t vec_gemm_smem_bytes(uint32_t d, bool ts) {
-    return (ts ? (size_t)STAGES_TS * B_BLOCK : (size_t)(d / GK) * A_BLOCK + STAGES * B_BLOCK) + 512 + 1023;  // + 1 KB static (row metadata)
+size_t vec_gemm_smem_bytes(uint32_t d) {
+    // query tile + B ring + accumulator staging + barriers + alignment slack (the 1 KB of row metadata is static)
+    return (size_t)(d / GK) * A_BLOCK + (size_t)STAGES * B_BLOCK + (size_t)NACC * ACC_BYTES + 256 + 1023;
 }
 
 bool vec_gemm_supported(uint32_t d, uint32_t limit) { return d % GK == 0 && d >= GK && d <= 768 && limit >= 1 && limit <= KMAX; }
@@ -735,45 +580,15 @@ cudaError_t launch_vec_gemm_topk(cudaStream_t s, uint32_t sm_count, const void *
     if (!vec_gemm_supported(d, k) || n_qtiles * n_groups > sm_count || n_groups == 0) return cudaErrorInvalidValue;
     CUtensorMap mq, mm;
     if (!make_map(&mq, q_fp16, (uint64_t)n_qtiles * GM, d, GM) || !make_map(&mm, mat_fp16, n_rows, d, GN)) return cudaErrorNotSupported;
-    cudaError_t em = cudaMemsetAsync(gthr, 0xff, (size_t)n_qtiles * GM * n_groups * 8, s);
-    if (em != cudaSuccess) return em;
-    unsigned long long *dbg = nullptr;
-    const uint32_t dbg_mode = getenv("B200_VEC_DEBUG") ? (uint32_t)atoi(getenv("B200_VEC_DEBUG")) : 0;
-    if (dbg_mode) {
-        if (cudaMalloc((void **)&dbg, (size_t)n_qtiles * n_groups * 64) != cudaSuccess) dbg = nullptr;
-        if (dbg) cudaMemsetAsync(dbg, 0, (size_t)n_qtiles * n_groups * 64, s);
-    }
-    // default: TMEM-resident query tile (deep matrix ring); B200_VEC_GEMM_TS=0 keeps the query tile in shared memory (k-split accumulators)
-    const bool ts = d % 64 == 0 && !(getenv("B200_VEC_GEMM_TS") && atoi(getenv("B200_VEC_GEMM_TS")) == 0);
-    size_t smem = vec_gemm_smem_bytes(d, ts);
-    const __half *qh = reinterpret_cast<const __half *>(q_fp16);
-    cudaError_t e;
-    if (ts) {
-        e = cudaFuncSetAttribute(vec_gemm_topk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        vec_gemm_topk_kernel<true><<<n_qtiles * n_groups, 256, smem, s>>>(mq, mm, qh, d, n_rows, d / GK, n_qtiles, n_groups, inv_norm, docids, q_inv_norm,
-                                                                          cand, n_cand_words, k, gthr, runs, partial, dbg, dbg_mode);
-    } else {
-        e = cudaFuncSetAttribute(vec_gemm_topk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        vec_gemm_topk_kernel<false><<<n_qtiles * n_groups, 256, smem, s>>>(mq, mm, qh, d, n_rows, d / GK, n_qtiles, n_groups, inv_norm, docids, q_inv_norm,
-                                                                           cand, n_cand_words, k, gthr, runs, partial, dbg, dbg_mode);
-    }
+    cudaError_t e = cudaMemsetAsync(gthr, 0xff, (size_t)n_qtiles * GM * n_groups * 8, s);
+    if (e != cudaSuccess) return e;
+    const size_t smem = vec_gemm_smem_bytes(d);
+    e = cudaFuncSetAttribute(vec_gemm_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    vec_gemm_topk_kernel<<<n_qtiles * n_groups, 256, smem, s>>>(mq, mm, n_rows, d / GK, n_qtiles, n_groups, inv_norm, docids, q_inv_norm, cand,
+                                                                n_cand_words, k, gthr, runs, partial);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    if (dbg) {
-        std::vector<unsigned long long> h((size_t)n_qtiles * n_groups * 8);
-        cudaStreamSynchronize(s);
-        cudaMemcpy(h.data(), dbg, h.size() * 8, cudaMemcpyDeviceToHost);
-        cudaFree(dbg);
-        double sum[8] = {0};
-        for (size_t c = 0; c < (size_t)n_qtiles * n_groups; c++)
-            for (int i = 0; i < 8; i++) sum[i] += (double)h[c * 8 + i];
-        const char *names[8] = {"epi tmem ld", dbg_mode == 2 ? "mma wait acc_empty" : "epi pass1", dbg_mode == 2 ? "mma wait b_full" : "epi pass2", "mma total", "warp0 flagged columns", "lane0 flagged", "epi compaction", "epi total"};
-        fprintf(stderr, "[b200 vec debug] mean cycles per CTA (%u CTAs):", n_qtiles * n_groups);
-        for (int i = 0; i < 8; i++) fprintf(stderr, "  %s %.0f", names[i], sum[i] / (n_qtiles * n_groups));
-        fprintf(stderr, "\n");
-    }
     vec_merge_kernel<<<n_q, KMAX, 0, s>>>(partial, n_groups, k, out_ids, out_dist, out_n);
     return cudaGetLastError();
 }

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path through the C ABI vs the CPU oracle and the
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path through the C ABI vs the CPU oracle and the
 reference goldens.  Integer/bit work must match exactly; vector scores within 1e-4 relative."""
 import numpy as np
 import pytest
@@ -114,7 +114,7 @@ def test_nns_matches_oracle(mb, synth):
 
 
 def test_nns_tensor_core_batch_matches_oracle(mb, synth, monkeypatch):
-    """The batched vector stage (tcgen05 GEMM + fused top-k) against the oracle and against the GEMV scan."""
+    """The batched vector stage (wgmma GEMM + fused top-k) against the oracle and against the GEMV scan."""
     from oracle.pyoracle import OracleIndex
 
     rng = np.random.default_rng(7)

@@ -32,7 +32,7 @@ for i in range(5):
 s = ix.stats()["kernels"]["vec_dist"]
 print("B=8: %.3f ms/launch, %.1f GB/s" % (s["ms"] / s["count"], s["bytes"] / (s["ms"] * 1e-3) / 1e9))
 
-# batched stage: tcgen05 GEMM + fused top-k
+# batched stage: wgmma GEMM + fused top-k
 for B in (128, 1024):
     qq = rng.standard_normal((B, d), dtype=np.float32)
     os.environ["B200_VEC_GEMM"] = "1"
@@ -43,5 +43,5 @@ for B in (128, 1024):
         ix.nns_by_vector(qq, 100)
     s = ix.stats()["kernels"]["vec_gemm_topk"]
     ms = s["ms"] / s["count"]
-    bp = (B + 127) // 128 * 128
+    bp = (B + 63) // 64 * 64
     print("B=%d gemm+merge: %.3f ms/launch, %.1f TFLOP/s (padded %d), %.0f queries/s kernel-only" % (B, ms, 2.0 * bp * n * d / (ms * 1e-3) / 1e12, bp, B / (ms * 1e-3)))
