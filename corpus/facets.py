@@ -1,0 +1,165 @@
+"""Facet databases in their LMDB byte formats (test/bench infrastructure): facet_id_f64_docids and facet_id_string_docids.
+
+Key: u16 BE fid | u8 level | bound (OrderedF64Codec, heed_codec/facet/ordered_f64_codec.rs, or the normalised string);
+value: FacetGroupValueCodec = u8 size | CBO roaring (heed_codec/facet/mod.rs).  Level-0 entries hold one value each; levels >= 1
+group FACET_GROUP_SIZE entries of the level below (left bound = the first one's) as the reference's incremental indexer does, so
+that readers which must ignore them see them.  JSON documents go through milli's extraction rules: arrays are flattened, `null`,
+objects and the empty string get no facet, booleans become the strings "true" / "false", strings are normalised (lib.rs:442)."""
+from __future__ import annotations
+
+import struct
+import unicodedata
+
+import numpy as np
+
+from .pyindexgen import DbImage
+
+FACET_GROUP_SIZE = 4
+
+
+def normalize_facet(s: str) -> str:
+    """lib.rs normalize_facet: NFKD (compatibility decomposition) of the trimmed string, lower-cased"""
+    return unicodedata.normalize("NFKD", s.strip()).lower()
+
+
+def ordered_f64(f: float) -> bytes:
+    """OrderedF64Codec: globally ordered bytes (facet/value_encoding.rs f64_into_bytes), then the f64 big-endian"""
+    f = float(f)
+    be = bytearray(struct.pack(">d", 0.0 if f == 0.0 else f))
+    if f < 0:
+        be = bytearray(b ^ 0xFF for b in be)
+    else:
+        be[0] ^= 0x80
+    return bytes(be) + struct.pack(">d", f)
+
+
+def cbo_encode(docids) -> bytes:
+    """CboRoaringBitmapCodec: <= 7 docids as raw native-endian u32, otherwise the portable roaring format without run containers"""
+    d = np.unique(np.asarray(docids, np.uint32))
+    if len(d) <= 7:
+        return d.astype("<u4").tobytes()
+    hi = d >> 16
+    keys, starts = np.unique(hi, return_index=True)
+    ends = list(starts[1:]) + [len(d)]
+    desc, bodies = [], []
+    for k, a, b in zip(keys, starts, ends):
+        lo = (d[a:b] & 0xFFFF).astype(np.uint16)
+        desc.append(struct.pack("<HH", int(k), len(lo) - 1))
+        if len(lo) <= 4096:
+            bodies.append(lo.astype("<u2").tobytes())
+        else:
+            words = np.zeros(1024, np.uint64)
+            np.bitwise_or.at(words, lo >> 6, np.left_shift(np.uint64(1), (lo & 63).astype(np.uint64)))
+            bodies.append(words.astype("<u8").tobytes())
+    n = len(keys)
+    head = struct.pack("<II", 12346, n) + b"".join(desc)
+    offs, at = [], len(head) + 4 * n
+    for body in bodies:
+        offs.append(struct.pack("<I", at))
+        at += len(body)
+    return head + b"".join(offs) + b"".join(bodies)
+
+
+def _db(entries):
+    """entries: sorted list of (key bytes, value bytes)"""
+    kb = b"".join(k for k, _ in entries)
+    vb = b"".join(v for _, v in entries)
+    ko = np.zeros(len(entries) + 1, np.uint64)
+    vo = np.zeros(len(entries) + 1, np.uint64)
+    ko[1:] = np.cumsum([len(k) for k, _ in entries]) if entries else []
+    vo[1:] = np.cumsum([len(v) for _, v in entries]) if entries else []
+    return DbImage(np.frombuffer(kb, np.uint8).copy(), ko, np.frombuffer(vb, np.uint8).copy(), vo)
+
+
+class FacetImage:
+    """Faceted fields of an index: field name -> fid, and per field the documents of every number / string value."""
+
+    def __init__(self):
+        self.fields = {}  # name -> fid
+        self.numbers = {}  # fid -> {float: [docids]}
+        self.strings = {}  # fid -> {normalised str: [docids]}
+
+    def fid(self, name):
+        if name not in self.fields:
+            self.fields[name] = len(self.fields)
+        return self.fields[name]
+
+    def add_facet(self, docid, name, value):
+        """one already-extracted facet value: a number (int/float) or a string (normalised here)"""
+        f = self.fid(name)
+        if isinstance(value, str):
+            v = normalize_facet(value)
+            if v:
+                self.strings.setdefault(f, {}).setdefault(v, []).append(docid)
+        else:
+            self.numbers.setdefault(f, {}).setdefault(float(value), []).append(docid)
+
+    def add_json(self, docid, name, value):
+        """a JSON field value through milli's facet extraction: arrays flattened; null / objects / "" give nothing"""
+        self.fid(name)
+        if isinstance(value, list):
+            for v in value:
+                self.add_json(docid, name, v)
+        elif isinstance(value, bool):
+            self.add_facet(docid, name, "true" if value else "false")
+        elif isinstance(value, (int, float)):
+            self.add_facet(docid, name, value)
+        elif isinstance(value, str):
+            self.add_facet(docid, name, value)
+
+    def add_synthetic(self, n_docs, seed=0x50A7):
+        """seeded facet fields: `price` (numbers with many duplicates, ~10 % missing), `brand` (Zipf-distributed strings), `tags`
+        (arrays of 1-3 mixed numbers and strings)"""
+        rng = np.random.default_rng(seed)
+        docs = np.arange(n_docs, dtype=np.uint32)
+        price = np.round(rng.gamma(2.0, 40.0, n_docs), 1)
+        has_price = rng.random(n_docs) >= 0.10
+        self._bulk("price", docs[has_price], price[has_price], numbers=True)
+        n_brands = 500
+        w = 1.0 / np.arange(1, n_brands + 1) ** 1.1
+        brand = rng.choice(n_brands, n_docs, p=w / w.sum())
+        has_brand = rng.random(n_docs) >= 0.05
+        names = np.array([f"brand{b:03d}" for b in range(n_brands)])
+        self._bulk("brand", docs[has_brand], names[brand[has_brand]], numbers=False)
+        n_tags = rng.integers(1, 4, n_docs)
+        for k in range(3):
+            sel = docs[n_tags > k]
+            is_num = rng.random(len(sel)) < 0.4
+            nums = rng.integers(0, 200, len(sel))
+            strs = np.array([f"tag{t:02d}" for t in range(60)])[rng.integers(0, 60, len(sel))]
+            self._bulk("tags", sel[is_num], nums[is_num].astype(np.float64), numbers=True)
+            self._bulk("tags", sel[~is_num], strs[~is_num], numbers=False)
+        return self
+
+    def _bulk(self, name, docids, values, numbers):
+        f = self.fid(name)
+        tab = (self.numbers if numbers else self.strings).setdefault(f, {})
+        order = np.argsort(values, kind="stable")
+        vals, starts = np.unique(values[order], return_index=True)
+        ends = list(starts[1:]) + [len(order)]
+        for v, a, b in zip(vals, starts, ends):
+            key = float(v) if numbers else normalize_facet(str(v))
+            tab.setdefault(key, []).extend(int(x) for x in docids[order[a:b]])
+
+    def build(self):
+        """-> (facet_id_f64_docids, facet_id_string_docids) as DbImage, keys in LMDB (bytewise) order"""
+        self.f64_db = _db(self._entries(self.numbers, lambda v: ordered_f64(v)))
+        self.string_db = _db(self._entries(self.strings, lambda v: v.encode()))
+        return self.f64_db, self.string_db
+
+    @staticmethod
+    def _entries(tab, enc):
+        out = []
+        for fid, vals in tab.items():
+            level = sorted((enc(v), np.unique(np.asarray(d, np.uint32))) for v, d in vals.items())
+            lv = 0
+            while level:
+                for bound, d in level:
+                    out.append((struct.pack(">HB", fid, lv) + bound, bytes([1 if lv == 0 else FACET_GROUP_SIZE]) + cbo_encode(d)))
+                if len(level) <= FACET_GROUP_SIZE:
+                    break
+                level = [(level[i][0], np.unique(np.concatenate([d for _, d in level[i:i + FACET_GROUP_SIZE]])))
+                         for i in range(0, len(level), FACET_GROUP_SIZE)]
+                lv += 1
+        out.sort(key=lambda e: e[0])
+        return out

@@ -20,7 +20,7 @@ extern "C" {
 #define B200_ERR_NO_DEVICE (-1)   /* no CUDA device / driver (the product never falls back to the CPU) */
 #define B200_ERR_CUDA (-2)        /* a CUDA call failed; see b200_last_error */
 #define B200_ERR_INVALID (-3)     /* bad argument */
-#define B200_ERR_UNSUPPORTED (-4) /* query feature outside the implemented scope (sort, filters, more than 12 terms, ...) */
+#define B200_ERR_UNSUPPORTED (-4) /* query feature outside the implemented scope (geo, distinct, more than 12 terms, ...) */
 #define B200_ERR_CAPACITY (-5)    /* a device work queue / arena overflowed */
 #define B200_ERR_STATE (-6)       /* call order (e.g. search before b200_stage_finish) */
 
@@ -49,7 +49,13 @@ enum b200_db {
     B200_DB_WORD_PREFIX_POSITION_DOCIDS = 7,
     B200_DB_WORD_PREFIX_FID_DOCIDS = 8,
     B200_DB_FIELD_ID_WORD_COUNT_DOCIDS = 9,/* key: u16 BE fid | u8 count */
-    B200_DB_COUNT = 10
+    /* facet databases read by the Sort rule (search/new/sort.rs:98-195).  Key: u16 BE fid | u8 level | left bound, where the bound
+     * is the 16-byte OrderedF64Codec (heed_codec/facet/ordered_f64_codec.rs: globally ordered f64 bytes, then the f64 big-endian)
+     * or the normalised string bytes (lib.rs normalize_facet; booleans are "true" / "false").  Value: FacetGroupValueCodec =
+     * u8 size | CBO bytes (heed_codec/facet/mod.rs).  Only level-0 entries are read; higher levels are accepted and ignored. */
+    B200_DB_FACET_ID_F64_DOCIDS = 10,
+    B200_DB_FACET_ID_STRING_DOCIDS = 11,
+    B200_DB_COUNT = 12
 };
 /* Replaces Index::words_fst (index.rs:1238): the FST enumerated once on the host into its sorted word list. */
 int b200_stage_dictionary(b200_index *, const uint8_t *word_bytes, const uint64_t *word_offsets, uint64_t n_words);
@@ -63,6 +69,9 @@ int b200_stage_documents_ids(b200_index *, const uint8_t *cbo, uint64_t len);
 /* criteria (crates/milli/src/criterion.rs:121-131) */
 enum b200_criterion { B200_C_WORDS = 0, B200_C_TYPO = 1, B200_C_PROXIMITY = 2, B200_C_ATTRIBUTE = 3, B200_C_ATTRIBUTE_RANK = 4,
                       B200_C_WORD_POSITION = 5, B200_C_SORT = 6, B200_C_EXACTNESS = 7 };
+/* custom criteria Criterion::Asc(field) / Desc(field) (criterion.rs:32-35), fid = the field's id in the facet databases */
+#define B200_C_ASC(fid) (0x10000 | (int32_t)(fid))
+#define B200_C_DESC(fid) (0x20000 | (int32_t)(fid))
 typedef struct {
     uint32_t n_fields;              /* searchable fields; fid = 0..n_fields-1 */
     const uint16_t *weights;        /* fieldids_weights_map: fid -> weight */
@@ -174,11 +183,28 @@ typedef struct {
     /* Search::ranking_score_threshold (bucket_sort.rs:188,221-224,293-296) */
     int32_t has_ranking_score_threshold;
     double ranking_score_threshold;
+    /* Search::sort_criteria (search/mod.rs:160): the `sort` list of query i is entries [sort_begin[i], sort_begin[i+1]) of
+     * sort_fid / sort_asc; sort_begin NULL = no `sort` anywhere.  sort_fid: the field's id in the facet databases, 0xFFFF for a
+     * field absent from the fields map (it sorts nothing: every document lands in the Null bucket).  Rules on a field already
+     * sorted earlier in the rule list are skipped by fid; 0xFFFF entries are never skipped, so the caller, which sees the names,
+     * leaves out an absent field whose name is already sorted (milli deduplicates by name); sort_asc: 1 Asc, 0 Desc.
+     * The sortable-attributes check and `_geoPoint` stay with the caller.  A non-empty list while the criteria lack `sort`
+     * (SortRankingRuleMissing, search/new/mod.rs:998-1040) is B200_ERR_INVALID for that query, in every mode.  Sort rules are
+     * implemented for placeholder searches of mode 0 only (no positive or negative query term: the rule stack is the sort rules
+     * alone, search/new/mod.rs:353-416).  B200_ERR_UNSUPPORTED for that query, never an answer without its sort rules: a sort rule
+     * (from the list or from Asc/Desc criteria) in a search with query terms or with negative terms only, in a semantic or hybrid
+     * search, more than B200_MAX_SCORES sort rules, `stop_after` together with a sort rule. */
+    const uint32_t *sort_begin;
+    const uint16_t *sort_fid;
+    const uint8_t *sort_asc;
 } b200_query_batch;
 #define B200_MAX_SCORES 12
 /* score kinds: ScoreDetails variants (score_details.rs:9-32) */
 enum b200_score_kind { B200_S_WORDS = 0, B200_S_TYPO = 1, B200_S_PROXIMITY = 2, B200_S_FID = 3, B200_S_POSITION = 4,
-                       B200_S_EXACT_ATTRIBUTE = 5, B200_S_EXACT_WORDS = 6, B200_S_VECTOR = 7, B200_S_SKIPPED = 8 };
+                       B200_S_EXACT_ATTRIBUTE = 5, B200_S_EXACT_WORDS = 6, B200_S_VECTOR = 7, B200_S_SKIPPED = 8, B200_S_SORT = 9 };
+/* B200_S_SORT (ScoreDetails::Sort, score_details.rs): score_max = fid << 2 | ascending << 1 | is_string; score_rank = position of
+ * the bucket's value among the staged level-0 keys of its database (facet_id_f64_docids when is_string = 0, else
+ * facet_id_string_docids), 0xFFFFFFFF for the Null bucket (no value).  Sort has no Rank: global scores ignore it. */
 typedef struct {                  /* SearchResult (search/mod.rs:526-535), flattened; all caller-allocated */
     uint32_t *docids;             /* n_queries x limit      documents_ids */
     uint32_t *n_hits;             /* n_queries */
@@ -226,7 +252,7 @@ void b200_rule_end(b200_rule *);
 /* ---- introspection for measurement ----------------------------------------------------- */
 /* kernel classes for the per-kernel accounting below */
 enum b200_kernel { B200_K_LEV = 0, B200_K_COMPACT = 1, B200_K_PAIR_PROBE = 2, B200_K_SCATTER = 3, B200_K_EVAL_PATHS = 4, B200_K_EMIT = 5,
-                   B200_K_VEC_DIST = 6, B200_K_TOPK = 7, B200_K_VEC_GEMM = 8, B200_K_VEC_MERGE = 9, B200_K_COUNT = 10 };
+                   B200_K_VEC_DIST = 6, B200_K_TOPK = 7, B200_K_VEC_GEMM = 8, B200_K_VEC_MERGE = 9, B200_K_SORT = 10, B200_K_COUNT = 11 };
 typedef struct {
     uint64_t kernel_launches;     /* kernels launched by the library since the last reset */
     uint64_t device_steps;        /* host<->device round trips since the last reset */
@@ -234,9 +260,9 @@ typedef struct {
     uint64_t matrix_bytes;        /* algorithmic bytes: condition/bucket matrix words read+written */
     uint64_t dictionary_bytes;    /* algorithmic bytes of the term-derivation sweeps */
     uint64_t vector_bytes;        /* algorithmic bytes of the distance scans */
-    double kernel_ms[10];         /* CUDA-event time accumulated per kernel class (events on the library's stream) */
-    uint64_t kernel_count[10];    /* launches per kernel class */
-    uint64_t kernel_bytes[10];    /* algorithmic bytes attributed to each kernel class */
+    double kernel_ms[B200_K_COUNT];      /* CUDA-event time accumulated per kernel class (events on the library's stream) */
+    uint64_t kernel_count[B200_K_COUNT]; /* launches per kernel class */
+    uint64_t kernel_bytes[B200_K_COUNT]; /* algorithmic bytes attributed to each kernel class */
     double device_ms;             /* CUDA-event time from the first to the last kernel of every step */
     uint64_t h2d_bytes, d2h_bytes; /* bytes copied across PCIe/NVLink-C2C by search/derive/nns calls */
     double host_ms[8];            /* wall time of the host phases of b200_search_batch: 0 parse, 1 derive (incl. device), 2 term finalisation,

@@ -22,7 +22,9 @@ MAX_SCORES = 12
 CRITERIA = {"words": 0, "typo": 1, "proximity": 2, "attribute": 3, "attributeRank": 4, "wordPosition": 5, "sort": 6, "exactness": 7}
 DEFAULT_CRITERIA = ["words", "typo", "proximity", "attributeRank", "sort", "wordPosition", "exactness"]  # criterion.rs:121-131
 TMS = {"last": 0, "all": 1, "frequency": 2}
-SCORE_KINDS = ["words", "typo", "proximity", "fid", "position", "exactAttribute", "exactWords", "vector", "skipped"]
+SCORE_KINDS = ["words", "typo", "proximity", "fid", "position", "exactAttribute", "exactWords", "vector", "skipped", "sort"]
+DB_FACET_F64, DB_FACET_STRING = 10, 11
+NO_FIELD = 0xFFFF  # a sort field absent from the fields map
 ERRORS = {-1: "NO_DEVICE", -2: "CUDA", -3: "INVALID", -4: "UNSUPPORTED", -5: "CAPACITY", -6: "STATE"}
 
 
@@ -44,7 +46,7 @@ class _Batch(C.Structure):
                 ("offset", C.c_uint32), ("limit", C.c_uint32), ("words_limit", C.c_uint32), ("vectors", C.c_void_p),
                 ("mode", C.c_int32), ("semantic_ratio", C.c_float), ("universes", C.c_void_p), ("n_universe_words", C.c_uint64),
                 ("time_budget_ns", C.c_uint64), ("stop_after", C.c_int64), ("has_ranking_score_threshold", C.c_int32),
-                ("ranking_score_threshold", C.c_double)]
+                ("ranking_score_threshold", C.c_double), ("sort_begin", C.c_void_p), ("sort_fid", C.c_void_p), ("sort_asc", C.c_void_p)]
 
 
 class _Results(C.Structure):
@@ -55,13 +57,13 @@ class _Results(C.Structure):
 
 class _Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("device_steps", C.c_uint64), ("posting_bytes", C.c_uint64), ("matrix_bytes", C.c_uint64),
-                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 10),
-                ("kernel_count", C.c_uint64 * 10), ("kernel_bytes", C.c_uint64 * 10), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
+                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 11),
+                ("kernel_count", C.c_uint64 * 11), ("kernel_bytes", C.c_uint64 * 11), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
                 ("hbm_bytes_staged", C.c_uint64), ("deferred", C.c_uint64), ("arena_peak_bytes", C.c_uint64),
                 ("eval_class_launches", C.c_uint64 * 9), ("eval_class_tiles", C.c_uint64 * 9)]
 
 
-KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge"]
+KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort"]
 
 
 def build_library(force=False):
@@ -129,7 +131,9 @@ def _p(a):
 class SearchResult:
     """milli::SearchResult (search/mod.rs:526-535) for a batch of queries."""
 
-    def __init__(self, n, limit):
+    def __init__(self, n, limit, sort_value=None):
+        self._sort_value = sort_value  # (fid, is_string, key index) -> (field name, value)
+        self.sort_names = None  # per query: the field name of each sort rule, in rule order
         self.limit = max(limit, 1)
         L = self.limit
         self.documents_ids = np.zeros((n, L), np.uint32)
@@ -158,6 +162,12 @@ class SearchResult:
                 if k == "vector":
                     sim = float(self.score_sim[q, i, s])
                     row.append(("vector", None if sim < 0 else sim))
+                elif k == "sort":
+                    m, key = int(self.score_max[q, i, s]), int(self.score_rank[q, i, s])
+                    field, value = self._sort_value(m >> 2, m & 1, key)
+                    if self.sort_names is not None and s < len(self.sort_names[q]):
+                        field = self.sort_names[q][s]  # the rule's field name (also for a field absent from the fields map)
+                    row.append(("sort", field, bool(m & 2), value))
                 else:
                     row.append((k, int(self.score_rank[q, i, s]), int(self.score_max[q, i, s])))
             out.append(row)
@@ -168,7 +178,7 @@ class Index:
     """The staged index: what milli reads from LMDB at query time, resident in HBM."""
 
     def __init__(self, image=None, *, device=0, criteria=None, authorize_typos=True, one_typo=5, two_typos=9, prefix_search=True,
-                 weights=None, exact_words=(), synonyms=None):
+                 weights=None, exact_words=(), synonyms=None, facets=None):
         self._l = load_library()
         h = C.c_void_p()
         rc = self._l.b200_open(device, C.byref(h))
@@ -178,24 +188,34 @@ class Index:
         self.dim = 0
         if image is not None:
             self.stage(image, criteria=criteria, authorize_typos=authorize_typos, one_typo=one_typo, two_typos=two_typos,
-                       prefix_search=prefix_search, weights=weights, exact_words=exact_words, synonyms=synonyms)
+                       prefix_search=prefix_search, weights=weights, exact_words=exact_words, synonyms=synonyms, facets=facets)
 
     def _ck(self, rc):
         if rc != 0:
             raise B200Error(rc, self._l.b200_last_error(self._h).decode())
 
     def stage(self, image, *, criteria=None, authorize_typos=True, one_typo=5, two_typos=9, prefix_search=True, weights=None, exact_words=(),
-              synonyms=None):
+              synonyms=None, facets=None):
         """image: anything with dict_bytes/dict_offsets/n_words, dbs[i].{key_bytes,key_offsets,val_bytes,val_offsets,n_keys},
-        documents_ids_cbo, n_fields — i.e. the LMDB databases in their on-disk formats."""
+        documents_ids_cbo, n_fields — i.e. the LMDB databases in their on-disk formats.  facets: a corpus.facets.FacetImage (or
+        anything with `fields` (name -> fid) and built `f64_db` / `string_db`); criteria may name custom rules "asc:<field>" /
+        "desc:<field>" (Criterion::Asc / Desc)."""
         l = self._l
+        self._facets = facets
+        self._fields = dict(facets.fields) if facets is not None else {}
+        self._level0 = {}  # (is_string) -> list of level-0 keys in staged order, for decoding Sort scores
+        if facets is not None:
+            for is_string, (dbid, db) in enumerate(((DB_FACET_F64, facets.f64_db), (DB_FACET_STRING, facets.string_db))):
+                self._ck(l.b200_stage_db(self._h, dbid, db.n_keys, _p(db.key_bytes), _p(db.key_offsets), _p(db.val_bytes), _p(db.val_offsets)))
+                self._level0[is_string] = [db.key(i) for i in range(db.n_keys) if db.key(i)[2] == 0]
         self._n_docs = int(image.n_docs)
         self._ck(l.b200_stage_dictionary(self._h, _p(image.dict_bytes), _p(image.dict_offsets), image.n_words))
         for i, db in enumerate(image.dbs):
             self._ck(l.b200_stage_db(self._h, i, db.n_keys, _p(db.key_bytes), _p(db.key_offsets), _p(db.val_bytes), _p(db.val_offsets)))
         self._ck(l.b200_stage_documents_ids(self._h, _p(image.documents_ids_cbo), len(image.documents_ids_cbo)))
         w = np.asarray(weights if weights is not None else list(range(image.n_fields)), np.uint16)
-        c = np.asarray([CRITERIA[x] for x in (DEFAULT_CRITERIA if criteria is None else criteria)], np.int32)
+        self._criteria_names = list(DEFAULT_CRITERIA if criteria is None else criteria)
+        c = np.asarray([self._criterion(x) for x in self._criteria_names], np.int32)
         s = _Settings(image.n_fields, _p(w), _p(c), len(c), int(authorize_typos), one_typo, two_typos, int(prefix_search),
                       "\n".join(exact_words).encode() if exact_words else None)
         self._ck(l.b200_stage_settings(self._h, C.byref(s)))
@@ -206,6 +226,44 @@ class Index:
             self._ck(l.b200_stage_synonyms(self._h, len(pairs), fr, to))
         self._ck(l.b200_stage_finish(self._h))
         self.n_fields = image.n_fields
+
+    def _criterion(self, name):
+        if name.startswith(("asc:", "desc:")):
+            d, field = name.split(":", 1)
+            return (0x10000 if d == "asc" else 0x20000) | self.field_id(field)
+        return CRITERIA[name]
+
+    def sort_rule_names(self, sort_list):
+        """field names of the sort rules of a search, in rule order (search/new/mod.rs:351-416, 651-716: the `sort` criterion expands
+        to the list once, Asc/Desc criteria add one rule each, a name already sorted is skipped) -> (names, the list's survivors)"""
+        names, kept, done = [], [], False
+        for c in self._criteria_names:
+            if c == "sort" and not done:
+                done = True
+                for item in sort_list:
+                    f = item.rsplit(":", 1)[0]
+                    if f not in names:
+                        names.append(f)
+                        kept.append(item)
+            elif c.startswith(("asc:", "desc:")):
+                f = c.split(":", 1)[1]
+                if f not in names:
+                    names.append(f)
+        return names, kept
+
+    def field_id(self, name):
+        """the field's id in the facet databases, NO_FIELD when the fields map lacks it"""
+        return self._fields.get(name, NO_FIELD)
+
+    def sort_value(self, fid, is_string, key_index):
+        """(field name, value) of a Sort score: the staged level-0 key's bound as a float or str, None for the Null bucket"""
+        import struct
+
+        name = next((n for n, f in self._fields.items() if f == fid), None)
+        if key_index == 0xFFFFFFFF:
+            return name, None
+        k = self._level0[is_string][key_index]
+        return name, (k[3:].decode() if is_string else struct.unpack(">d", k[11:19])[0])
 
     def set_embeddings(self, matrix, docids=None, distribution=None):
         """f32 rows (converted to fp16 on the device), or a float16 matrix staged as it is."""
@@ -376,6 +434,7 @@ class Search:
         self._scoring = "skip"
         self._offset, self._limit, self._words_limit = 0, 20, 10
         self._universes, self._budget_ms, self._stop_after, self._threshold, self._want_candidates = None, None, None, None, False
+        self._sort = None
 
     def query(self, queries, stop_words=frozenset()):
         self._tokens = queries if isinstance(queries, TokenBatch) else TokenBatch([queries] if isinstance(queries, str) else list(queries), stop_words)
@@ -419,6 +478,11 @@ class Search:
         self._threshold = t
         return self
 
+    def sort(self, criteria):
+        """Search::sort_criteria: ["price:asc", "brand:desc", ...] for every query of the batch, or one such list per query"""
+        self._sort = criteria
+        return self
+
     def with_candidates(self):
         self._want_candidates = True
         return self
@@ -430,7 +494,7 @@ class Search:
             n = self._vectors.shape[0] if self._vectors is not None else 1
             tokens = TokenBatch([""] * n)
         n = tokens.n_queries
-        res = SearchResult(n, self._limit)
+        res = SearchResult(n, self._limit, ix.sort_value)
         b = _Batch(n, _p(tokens.token_begin), _p(tokens.token_kind), _p(tokens.lemma_off), _p(tokens.lemma_bytes), TMS[self._tms],
                    1 if self._scoring == "detailed" else 0, self._offset, self._limit, self._words_limit,
                    _p(self._vectors) if self._vectors is not None else None, mode, ratio)
@@ -453,6 +517,20 @@ class Search:
                 b.n_universe_words = len(a)
             keep.append(ptrs)
             b.universes = C.cast(ptrs, C.c_void_p)
+        if self._sort is not None:
+            per_q = self._sort if (self._sort and isinstance(self._sort[0], (list, tuple))) else [self._sort] * n
+            rules = [ix.sort_rule_names(list(x)) for x in per_q]
+            res.sort_names = [r_[0] for r_ in rules]
+            # the library deduplicates by field id; a repeated name of a field absent from the fields map is dropped here
+            if "sort" in ix._criteria_names:  # (without it the list is SortRankingRuleMissing: sent as it is)
+                per_q = [kept if any(ix.field_id(i.rsplit(":", 1)[0]) == NO_FIELD for i in x) else list(x) for x, (_, kept) in zip(per_q, rules)]
+            begin = np.zeros(n + 1, np.uint32)
+            begin[1:] = np.cumsum([len(x) for x in per_q])
+            items = [c.rsplit(":", 1) for x in per_q for c in x]
+            fid = np.asarray([ix.field_id(f) for f, _ in items] or [0], np.uint16)
+            asc = np.asarray([1 if d == "asc" else 0 for _, d in items] or [0], np.uint8)
+            keep += [begin, fid, asc]
+            b.sort_begin, b.sort_fid, b.sort_asc = _p(begin), _p(fid), _p(asc)
         b.time_budget_ns = 0 if self._budget_ms is None else max(1, int(self._budget_ms * 1e6))
         b.stop_after = -1 if self._stop_after is None else int(self._stop_after)
         b.has_ranking_score_threshold = int(self._threshold is not None)

@@ -139,4 +139,19 @@ struct CompactTile {
     uint32_t n_seg;
 };
 
+// one window of a sort activation (sort.cu): the documents of ranks [lo, hi) of the universe ordered by (key_0, ..., key_{L-1}, docid)
+constexpr uint32_t SORT_MAX_LEVELS = 12;  // B200_MAX_SCORES
+constexpr uint32_t SORT_WINDOW = 2048;    // rows one CTA produces
+struct SortDesc {
+    const unsigned long long *ub;          // dense universe bitmap, n_words words
+    const uint32_t *keys[SORT_MAX_LEVELS]; // per level: u32[n_docs] sort keys, nullptr = every key 0 (a field without values)
+    uint32_t bits[SORT_MAX_LEVELS + 1];    // significant bits of each tuple word ([n_levels]: the docid)
+    uint32_t n_words, n_levels;
+    uint32_t lo, hi;                       // hi - lo <= SORT_WINDOW, hi <= |universe|
+    uint32_t *dst;                         // hi - lo docids
+    uint32_t *dst_keys;                    // (hi - lo) x n_levels keys
+    uint32_t *info;                        // out: universe passes, documents collected for the window
+};
+
 }  // namespace b200
+

@@ -380,7 +380,7 @@ struct Engine {
     // staging inputs
     std::vector<uint8_t> raw_dict_bytes;
     std::vector<uint64_t> raw_dict_off;
-    RawDb raw_dbs[10];
+    RawDb raw_dbs[B200_DB_COUNT];
     std::vector<uint8_t> raw_docids;
     bool staged = false;
     HostIndex hix;
@@ -420,6 +420,8 @@ struct Engine {
     DevBuf<uint32_t> d_qcount;   // [0] scatter jobs, [1] surviving paths
     DevBuf<PathOut> d_pathbuf;
     DevBuf<uint32_t> d_docids_out;  // n_queries x limit
+    DevBuf<SortDesc> d_sort_desc;   // sort windows of a batch (sort.cu)
+    DevBuf<uint32_t> d_sort_keys, d_sort_info;
     DevBuf<unsigned long long> d_universes;  // the batch's distinct filtered universes (documents_ids & filter), n_words64 words each
     DevBuf<uint32_t> d_rowtab;      // n_queries x n_words64: word -> (tag, row) of the query's current activation (ActDesc::row_tab)
     uint8_t *h_step = nullptr;      // pinned

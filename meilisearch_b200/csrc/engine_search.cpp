@@ -471,6 +471,16 @@ struct QState {
     const unsigned long long *cand_src = nullptr;  // device bitmap to copy into b200_results::candidates at the lane's next step
     std::vector<uint64_t> term_freq;  // Frequency: documents per term id, filled one device step per term before anything else
     uint32_t n_term_ids = 0;
+    // Sort rules of a placeholder search (search/new/mod.rs:351-416): fid and direction per rule; sort_lo/hi: the ranks of the
+    // universe the result window holds, produced by sort_window_kernel after the step loop
+    struct SortRule {
+        uint16_t fid;
+        bool asc;
+    };
+    std::vector<SortRule> sort_rules;
+    bool sort_pending = false;
+    uint32_t sort_lo = 0, sort_hi = 0;
+    std::vector<uint32_t> sort_ids;  // the result window's docids
     // arena blocks of levels bucket_sort has left; the lane's driver returns them to its allocator at the start of its next step
     // (the emissions queued by the same advance() still read them: they run first on the lane's stream, before any new owner writes)
     std::vector<std::pair<size_t, size_t>> freed;
@@ -1677,7 +1687,7 @@ uint8_t score_kind_of(int rk) {
 double global_score_of(const std::vector<EScore> &sc) {
     uint64_t rk = 1, mx = 1;
     for (auto &x : sc) {
-        if (x.kind == B200_S_VECTOR) continue;
+        if (x.kind == B200_S_VECTOR || x.kind == B200_S_SORT) continue;  // no Rank (score_details.rs:110-154)
         rk = rk > 0 ? rk - 1 : 0;
         rk = rk * x.max_rank + x.rank;
         mx *= x.max_rank;
@@ -1790,6 +1800,64 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         }
     });
     stats.host_ms[0] += ms_since(t_ph);
+    // ---- sort rules (search/new/mod.rs:351-416, 651-716): the `Sort` criterion expands to the query's `sort` list at its position,
+    // once; Asc(f) / Desc(f) criteria add one rule each; a field sorted earlier in the list is skipped
+    {
+        bool has_sort_criterion = false, has_custom = false;
+        for (int c : hix.settings.criteria) {
+            has_sort_criterion |= c == B200_C_SORT;
+            has_custom |= (c & 0x30000) != 0;
+        }
+        if (b->sort_begin || has_custom)
+            for (uint32_t i = 0; i < NQ; i++) {
+                QState &q = *qs[i];
+                if (q.done) continue;
+                const uint32_t s0 = b->sort_begin ? b->sort_begin[i] : 0, s1_ = b->sort_begin ? b->sort_begin[i + 1] : 0;
+                auto refuse = [&](int code, const char *why) {
+                    q.status = code;
+                    q.error = why;
+                    q.done = true;
+                };
+                if (s1_ > s0 && !has_sort_criterion) {  // check_sort_criteria (search/new/mod.rs:998-1016)
+                    refuse(B200_ERR_INVALID, "SortRankingRuleMissing: a sort list was given but the ranking rules do not contain `sort`");
+                    continue;
+                }
+                if (s1_ > s0 && (!b->sort_fid || !b->sort_asc)) {
+                    refuse(B200_ERR_INVALID, "sort_begin without sort_fid / sort_asc");
+                    continue;
+                }
+                std::vector<QState::SortRule> sr;
+                std::vector<uint16_t> sorted;
+                bool sort_done = false;
+                auto add = [&](uint16_t fid, bool asc) {
+                    // 0xFFFF stands for every field absent from the fields map: its entries are never "already sorted" (the caller,
+                    // which sees the names, drops a repeated absent name)
+                    if (fid != 0xFFFF && std::find(sorted.begin(), sorted.end(), fid) != sorted.end()) return;
+                    sorted.push_back(fid);
+                    sr.push_back(QState::SortRule{fid, asc});
+                };
+                for (int c : hix.settings.criteria) {
+                    if (c == B200_C_SORT && !sort_done) {
+                        sort_done = true;
+                        for (uint32_t k = s0; k < s1_; k++) add(b->sort_fid[k], b->sort_asc[k] != 0);
+                    } else if (c & 0x10000)
+                        add((uint16_t)(c & 0xffff), true);
+                    else if (c & 0x20000)
+                        add((uint16_t)(c & 0xffff), false);
+                }
+                if (sr.empty()) continue;
+                if (b->mode != 0)
+                    refuse(B200_ERR_UNSUPPORTED, "sort in a semantic or hybrid search (needs the ScoreValue::Sort comparator of hybrid.rs)");
+                else if (!q.placeholder)
+                    refuse(B200_ERR_UNSUPPORTED, "sort rule in a search with query terms (sort is built for placeholder searches)");
+                else if (sr.size() > B200_MAX_SCORES)
+                    refuse(B200_ERR_UNSUPPORTED, "more than B200_MAX_SCORES sort rules");
+                else if (b->stop_after >= 0)
+                    refuse(B200_ERR_UNSUPPORTED, "stop_after together with a sort rule (the sort window is one device step; its polls are not counted)");
+                else
+                    q.sort_rules = std::move(sr);
+            }
+    }
     // ---- filtered universes (search/new/mod.rs:719): every distinct bitmap is intersected with documents_ids and uploaded once
     const bool has_thr = b->has_ranking_score_threshold != 0;
     const double thr = b->ranking_score_threshold;
@@ -2036,6 +2104,37 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             finish_state_graph(L, ae, 0, 1, false);
             L.next_max_cost = 1;
             request_activation(q, std::move(L), nullptr, q.d_univ ? q.d_univ : dix.base_ub, nullptr, hix.n_words64, hix.n_words64, 0, hix.n_words64);
+            return;
+        }
+        if (q.placeholder && !q.sort_rules.empty()) {
+            // placeholder search ordered by its sort rules: the window [offset, offset + limit) of the universe in (keys, docid) order,
+            // one sort_window_kernel launch after the step loop.  Deadline::exceeded() is polled before the first bucket request
+            // (bucket_sort.rs:206-264): when the budget is already spent the universe is returned as it is, Skipped and degraded.
+            q.n_candidates = q.univ_count;
+            q.cand_src = q.d_univ ? q.d_univ : dix.base_ub;
+            uint64_t avail = q.univ_count > from ? q.univ_count - from : 0;
+            uint32_t take = (uint32_t)std::min<uint64_t>(avail, length);
+            if (has_budget && clk::now() >= deadline_at) {
+                q.degraded = true;
+                EmitReq e{};
+                e.d.uw = nullptr;
+                e.d.ub = q.d_univ ? q.d_univ : dix.base_ub;
+                e.d.out = nullptr;
+                e.d.rows = hix.n_words64;
+                e.d.ld = hix.n_words64;
+                e.d.skip = from;
+                e.d.take = take;
+                q.n_results = take;
+                q.scores.assign(take, std::vector<EScore>{EScore{B200_S_SKIPPED, 0, 1, -1.f}});
+                if (take) q.emits.push_back(e);
+            } else {
+                q.n_results = take;
+                q.scores.assign(take, {});
+                q.sort_pending = take > 0;
+                q.sort_lo = from;
+                q.sort_hi = from + take;
+            }
+            q.done = true;
             return;
         }
         if (q.placeholder) {
@@ -3175,6 +3274,129 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         if (lanes[l].rc < 0) return lanes[l].rc;
     if (r->candidates)
         for (unsigned l = 0; l < n_lanes; l++) CU(cudaStreamSynchronize(lanes[l].stream), "sync candidates");
+    // ---- sort windows of the placeholder searches with sort rules (sort.cu), on the handle's stream
+    {
+        std::vector<SortDesc> descs;
+        std::vector<std::pair<uint32_t, uint32_t>> owner;  // per window: query, first result row
+        size_t key_words = 0;
+        const uint32_t doc_bits = hix.n_docs > 1 ? 32u - (uint32_t)__builtin_clz(hix.n_docs - 1) : 0u;
+        // A query's ranks [sort_lo, sort_hi) are produced with one more rank on each side where the universe has it: under Skip a
+        // bucket of at most one document is returned with the scores of the rules above it only (bucket_sort.rs:299-312), and
+        // whether a document's group of equal keys is a singleton shows in its neighbours.
+        std::vector<uint32_t> q_first(NQ, 0), q_elo(NQ, 0);
+        size_t id_words = 0;
+        for (uint32_t i = 0; i < NQ; i++) {
+            QState &q = *qs[i];
+            if (!q.sort_pending || q.status != 0) continue;
+            const uint32_t L = (uint32_t)q.sort_rules.size();
+            const uint32_t elo = q.sort_lo > 0 ? q.sort_lo - 1 : 0, ehi = (uint32_t)std::min<uint64_t>(q.univ_count, (uint64_t)q.sort_hi + 1);
+            q_first[i] = (uint32_t)descs.size();
+            q_elo[i] = elo;
+            for (uint32_t lo = elo; lo < ehi; lo += SORT_WINDOW) {
+                SortDesc d{};
+                d.ub = q.d_univ ? q.d_univ : dix.base_ub;
+                d.n_words = hix.n_words64;
+                d.n_levels = L;
+                for (uint32_t l = 0; l < L; l++) {
+                    auto it = hix.sort_fields.find(q.sort_rules[l].fid);
+                    if (it == hix.sort_fields.end()) continue;  // no value anywhere: one Null bucket
+                    const uint32_t V = it->second.n_values();
+                    d.keys[l] = it->second.d_key[q.sort_rules[l].asc ? 0 : 1];
+                    d.bits[l] = V ? 32u - (uint32_t)__builtin_clz(V) : 0u;
+                }
+                d.bits[L] = doc_bits;
+                d.lo = lo;
+                d.hi = std::min<uint32_t>(ehi, lo + SORT_WINDOW);
+                d.dst = reinterpret_cast<uint32_t *>((uintptr_t)id_words);  // offsets, made pointers below
+                id_words += d.hi - d.lo;
+                d.dst_keys = reinterpret_cast<uint32_t *>((uintptr_t)key_words);  // offset, made a pointer below
+                key_words += (size_t)(d.hi - d.lo) * L;
+                descs.push_back(d);
+                owner.emplace_back(i, lo - elo);
+            }
+        }
+        if (!descs.empty()) {
+            const size_t n = descs.size();
+            CU(d_sort_keys.reserve(std::max<size_t>(1, key_words + id_words)), "alloc sort keys");
+            CU(d_sort_info.reserve(2 * n), "alloc sort info");
+            CU(d_sort_desc.reserve(n), "alloc sort windows");
+            for (size_t k = 0; k < n; k++) {
+                descs[k].dst_keys = d_sort_keys.p + (uintptr_t)descs[k].dst_keys;
+                descs[k].dst = d_sort_keys.p + key_words + (uintptr_t)descs[k].dst;
+                descs[k].info = d_sort_info.p + 2 * k;
+            }
+            CU(cudaMemcpyAsync(d_sort_desc.p, descs.data(), n * sizeof(SortDesc), cudaMemcpyHostToDevice, stream), "H2D sort windows");
+            const size_t m0 = mark();
+            CU(launch_sort_window(stream, d_sort_desc.p, (uint32_t)n), "sort_window");
+            time_kernel(B200_K_SORT, m0, mark(), 0);
+            std::vector<uint32_t> keys(key_words + id_words), info(2 * n);
+            CU(cudaMemcpyAsync(keys.data(), d_sort_keys.p, (key_words + id_words) * 4, cudaMemcpyDeviceToHost, stream), "D2H sort keys");
+            CU(cudaMemcpyAsync(info.data(), d_sort_info.p, 2 * n * 4, cudaMemcpyDeviceToHost, stream), "D2H sort info");
+            CU(cudaStreamSynchronize(stream), "sync sort");
+            resolve_timers();
+            stats.h2d_bytes += n * sizeof(SortDesc);
+            stats.d2h_bytes += (key_words + id_words) * 4 + 2 * n * 4;
+            for (size_t k = 0; k < n; k++) {
+                const SortDesc &d = descs[k];
+                QState &q = *qs[owner[k].first];
+                const uint32_t rows = d.hi - d.lo, L = d.n_levels;
+                // algorithmic bytes: every pass reads the universe words and one key per document; the window writes docids + keys
+                stats.kernel_bytes[B200_K_SORT] += (uint64_t)info[2 * k] * (hix.n_words64 * 8ull + q.univ_count * 4ull) + (uint64_t)rows * 4 * (L + 1);
+                if (info[2 * k + 1] != rows) {
+                    q.status = B200_ERR_CUDA;
+                    q.error = "internal: sort window collected a different number of documents than its rank range";
+                }
+            }
+            for (uint32_t i = 0; i < NQ; i++) {
+                QState &q = *qs[i];
+                if (!q.sort_pending || q.status != 0) continue;
+                const SortDesc &d0 = descs[q_first[i]];
+                const uint32_t L = d0.n_levels, elo = q_elo[i];
+                const uint32_t n_ext = (uint32_t)std::min<uint64_t>(q.univ_count, (uint64_t)q.sort_hi + 1) - elo;
+                const uint32_t *ids = keys.data() + key_words + ((uintptr_t)d0.dst - (uintptr_t)(d_sort_keys.p + key_words)) / 4;
+                const uint32_t *kp = keys.data() + ((uintptr_t)d0.dst_keys - (uintptr_t)d_sort_keys.p) / 4;
+                auto shares = [&](uint32_t a, uint32_t b, uint32_t n_keys) {  // keys [0, n_keys) of ext rows a and b agree
+                    for (uint32_t l = 0; l < n_keys; l++)
+                        if (kp[(size_t)a * L + l] != kp[(size_t)b * L + l]) return false;
+                    return true;
+                };
+                q.sort_ids.assign(ids + (q.sort_lo - elo), ids + (q.sort_hi - elo));
+                for (uint32_t j = 0; j < q.sort_hi - q.sort_lo; j++) {
+                    const uint32_t e = q.sort_lo - elo + j;
+                    // Under Skip a document leaves bucket_sort early at the first rule l (top down) where either
+                    //  - the rule's remaining universe is that document alone (bucket_sort.rs:196-204): it is the last of its group of
+                    //    equal keys [0, l) and no other document of that group shares its key l -> the scores of the rules above l;
+                    //  - the rule's bucket holding it has no other document (:299-312) -> the scores of rules [0, l].
+                    uint32_t n_sc = L;
+                    if (skip_scoring)
+                        for (uint32_t l = 0; l < L; l++) {
+                            const bool has_prev = e > 0, has_next = e + 1 < n_ext;
+                            const bool last_of_group = !(has_next && shares(e, e + 1, l));
+                            const bool alone = !(has_prev && shares(e, e - 1, l + 1)) && !(has_next && shares(e, e + 1, l + 1));
+                            if (last_of_group && alone) {
+                                n_sc = l;
+                                break;
+                            }
+                            if (alone) {
+                                n_sc = l + 1;
+                                break;
+                            }
+                        }
+                    std::vector<EScore> &sc = q.scores[j];
+                    sc.clear();
+                    for (uint32_t l = 0; l < n_sc; l++) {
+                        const QState::SortRule &rule = q.sort_rules[l];
+                        const uint32_t key = kp[(size_t)e * L + l];
+                        auto it = hix.sort_fields.find(rule.fid);
+                        bool is_string = false;
+                        uint32_t key_index = 0xffffffffu;
+                        if (it != hix.sort_fields.end() && key < it->second.n_values()) it->second.decode(rule.asc, key, is_string, key_index);
+                        sc.push_back(EScore{B200_S_SORT, key_index, (uint32_t)rule.fid << 2 | (rule.asc ? 2u : 0u) | (is_string ? 1u : 0u), -1.f});
+                    }
+                }
+            }
+        }
+    }
     // ---- outputs
     t_ph = clk::now();
     std::vector<uint32_t> out_ids((size_t)NQ * std::max(1u, length));
@@ -3192,6 +3414,8 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             continue;
         }
         r->n_hits[i] = q.n_results;
+        if (q.sort_pending)
+            for (uint32_t k = 0; k < q.n_results; k++) out_ids[(size_t)i * std::max(1u, length) + k] = q.sort_ids[k];
         if (r->n_candidates) r->n_candidates[i] = q.n_candidates;
         if (r->degraded) r->degraded[i] = q.degraded ? 1 : 0;
         if (r->used_negative_operator) r->used_negative_operator[i] = q.used_negative ? 1 : 0;

@@ -88,6 +88,9 @@ Engine::~Engine() {
     for (void *p : {(void *)dix.dict_bytes, (void *)dix.dict_off, (void *)dix.pool, (void *)dix.lists, (void *)dix.pair_keys, (void *)dix.base_ub,
                     (void *)dix.emb, (void *)dix.emb_inv_norm, (void *)dix.emb_docids, (void *)arena, (void *)scratch})
         if (p) cudaFree(p);
+    for (auto &kv : hix.sort_fields)
+        for (auto p : kv.second.d_key)
+            if (p) cudaFree(p);
     for (auto &ln : lanes) ln.release();
     d_step.release();
     d_results.release();
@@ -95,6 +98,9 @@ Engine::~Engine() {
     d_qcount.release();
     d_pathbuf.release();
     d_docids_out.release();
+    d_sort_desc.release();
+    d_sort_keys.release();
+    d_sort_info.release();
     d_lev_terms.release();
     d_lev_recs.release();
     d_lev_u32.release();
@@ -140,6 +146,7 @@ int Engine::stage_finish() {
     CU(cudaSetDevice(device), "cudaSetDevice");
     try {
         build_host_index(raw_dict_bytes, raw_dict_off, raw_dbs, raw_docids, hix);
+        build_sort_fields(raw_dbs[B200_DB_FACET_ID_F64_DOCIDS], raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], hix);
     } catch (const std::exception &e) {
         return fail(B200_ERR_INVALID, e.what());
     }
@@ -160,6 +167,14 @@ int Engine::stage_finish() {
     stats.hbm_bytes_staged = hix.dict_bytes.size() + off32.size() * 4 + hix.pool.size() * 4 + hix.lists.size() * sizeof(ListRef) +
                              hix.pair_keys.size() * 8 + hix.base_ub.size() * 8;
     std::vector<uint32_t>().swap(hix.pool);
+    // Sort keys: two u32[n_docs] per faceted field (ascending, descending)
+    for (auto &kv : hix.sort_fields)
+        for (int dir = 0; dir < 2; dir++) {
+            std::vector<uint32_t> &k = kv.second.key[dir];
+            CU(upload(&kv.second.d_key[dir], k.data(), k.size()), "upload sort keys");
+            stats.hbm_bytes_staged += k.size() * 4;
+            std::vector<uint32_t>().swap(k);
+        }
     // release the raw staging copies
     for (auto &db : raw_dbs) {
         std::vector<uint8_t>().swap(db.keys);

@@ -308,4 +308,68 @@ void build_host_index(const std::vector<uint8_t> &dict_bytes, const std::vector<
     }
 }
 
+void build_sort_fields(const RawDb &f64_db, const RawDb &string_db, HostIndex &ix) {
+    ix.sort_fields.clear();
+    struct Val {
+        uint16_t fid;
+        uint32_t key_index;  // among the level-0 keys of its database
+        std::vector<uint32_t> docs;
+    };
+    // level-0 entries in LMDB order (u16 BE fid | u8 level | bound): per field, numbers and strings each come in ascending order
+    auto level0 = [&](const RawDb &db, bool numbers) {
+        std::vector<Val> out;
+        uint32_t l0 = 0;
+        for (uint64_t i = 0; i < db.n; i++) {
+            const uint8_t *k = db.keys.data() + db.koff[i];
+            size_t kn = db.koff[i + 1] - db.koff[i];
+            if (kn < 3) throw std::runtime_error("stage: facet key shorter than fid + level");
+            if (k[2] != 0) continue;  // group levels: only level 0 is read
+            if (numbers && kn != 3 + 16) throw std::runtime_error("stage: facet_id_f64_docids key without a 16-byte OrderedF64 bound");
+            const uint8_t *v = db.vals.data() + db.voff[i];
+            size_t vn = db.voff[i + 1] - db.voff[i];
+            if (vn < 1) throw std::runtime_error("stage: facet value without its group size byte");
+            Val x;
+            x.fid = (uint16_t)(k[0] << 8 | k[1]);
+            x.key_index = l0++;
+            cbo_decode_append(v + 1, vn - 1, x.docs);
+            out.push_back(std::move(x));
+        }
+        return out;
+    };
+    std::vector<Val> nums = level0(f64_db, true), strs = level0(string_db, false);
+    for (auto &x : nums) {
+        SortField &f = ix.sort_fields[x.fid];
+        f.num_key.push_back(x.key_index);
+        f.n_num++;
+    }
+    for (auto &x : strs) {
+        SortField &f = ix.sort_fields[x.fid];
+        f.str_key.push_back(x.key_index);
+        f.n_str++;
+    }
+    for (auto &kv : ix.sort_fields) {
+        SortField &f = kv.second;
+        f.key[0].assign(ix.n_docs, f.n_values());
+        f.key[1].assign(ix.n_docs, f.n_values());
+    }
+    // ordinal of the i-th number / j-th string of a field in each direction; a document keeps the smallest (its first bucket)
+    std::map<uint16_t, uint32_t> seen;
+    auto fold = [&](std::vector<Val> &vals, bool numbers) {
+        seen.clear();
+        for (auto &x : vals) {
+            SortField &f = ix.sort_fields[x.fid];
+            uint32_t i = seen[x.fid]++;
+            uint32_t oa = numbers ? i : f.n_num + i;
+            uint32_t od = numbers ? f.n_num - 1 - i : f.n_num + (f.n_str - 1 - i);
+            for (uint32_t d : x.docs) {
+                if (d >= ix.n_docs) continue;  // not in documents_ids
+                f.key[0][d] = std::min(f.key[0][d], oa);
+                f.key[1][d] = std::min(f.key[1][d], od);
+            }
+        }
+    };
+    fold(nums, true);
+    fold(strs, false);
+}
+
 }  // namespace b200

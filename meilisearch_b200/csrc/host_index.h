@@ -49,6 +49,27 @@ struct Settings {
 
 constexpr uint32_t NO_LIST = 0xffffffffu;
 
+// One faceted field as the Sort rule sees it (search/new/sort.rs:98-195 over the level-0 entries of facet_id_f64_docids and
+// facet_id_string_docids).  Its values are numbered in the order a sort walks them: ascending = numbers ascending, then strings
+// ascending; descending = numbers descending, then strings descending (numbers still first).  key[dir][doc] is the smallest
+// ordinal among the document's values, n_values() when it has none: the Sort buckets of any universe are the groups of equal key
+// in ascending key order (DESIGN.md §3).
+struct SortField {
+    uint32_t n_num = 0, n_str = 0;
+    std::vector<uint32_t> num_key, str_key;  // value i -> position among the staged level-0 keys of its database
+    std::vector<uint32_t> key[2];            // [0] ascending, [1] descending: u32[n_docs], released after upload
+    uint32_t *d_key[2] = {nullptr, nullptr}; // the same in HBM
+    uint32_t n_values() const { return n_num + n_str; }
+    // ordinal of direction `asc` -> (is_string, position among the level-0 keys of its database)
+    void decode(bool asc, uint32_t o, bool &is_string, uint32_t &key_index) const {
+        is_string = o >= n_num;
+        if (!is_string)
+            key_index = num_key[asc ? o : n_num - 1 - o];
+        else
+            key_index = str_key[asc ? o - n_num : n_str - 1 - (o - n_num)];
+    }
+};
+
 struct HostIndex {
     // dictionary
     std::vector<uint8_t> dict_bytes;
@@ -73,6 +94,7 @@ struct HostIndex {
     std::vector<uint64_t> pair_keys;
     uint32_t pair_list_base = 0;
     std::map<uint32_t, uint32_t> fwc_list;  // fid<<8|count -> list
+    std::map<uint16_t, SortField> sort_fields;  // faceted fields (fid -> SortField)
     // list id of key i of database db = db_first[db] + i (keys in LMDB order); db_keys[db] = number of staged keys.
     // (word_pair_proximity keys naming unknown words are dropped at staging: for that db the mapping only holds when none was.)
     uint32_t db_first[10] = {0}, db_keys[10] = {0};
@@ -169,5 +191,8 @@ struct HostIndex {
 // Decode the staged LMDB-format databases into `out` (directories + pool). Throws std::runtime_error.
 void build_host_index(const std::vector<uint8_t> &dict_bytes, const std::vector<uint64_t> &dict_off, const RawDb *dbs /*[10]*/,
                       const std::vector<uint8_t> &docids_cbo, HostIndex &out);
+// Decode the level-0 entries of facet_id_f64_docids / facet_id_string_docids into out.sort_fields (after build_host_index: needs
+// n_docs).  Throws std::runtime_error on a malformed key or value.
+void build_sort_fields(const RawDb &f64_db, const RawDb &string_db, HostIndex &out);
 
 }  // namespace b200
