@@ -61,8 +61,7 @@ int b200_open(int device_ordinal, b200_index **out) {
     if (!h) return B200_ERR_INVALID;
     h->e.device = device_ordinal;
     if ((err = cudaSetDevice(device_ordinal)) != cudaSuccess || (err = cudaStreamCreateWithFlags(&h->e.stream, cudaStreamNonBlocking)) != cudaSuccess ||
-        (err = cudaStreamCreateWithFlags(&h->e.vt.stream, cudaStreamNonBlocking)) != cudaSuccess ||
-        (err = cudaEventCreate(&h->e.ev0)) != cudaSuccess || (err = cudaEventCreate(&h->e.ev1)) != cudaSuccess) {
+        (err = cudaStreamCreateWithFlags(&h->e.vt.stream, cudaStreamNonBlocking)) != cudaSuccess) {
         g_open_error = std::string("CUDA init failed: ") + cudaGetErrorString(err);
         delete h;
         return B200_ERR_CUDA;
@@ -453,28 +452,17 @@ int Engine::search_batch(const b200_query_batch *b, b200_results *r) {
         // Sort rules in a semantic search (get_ranking_rules_for_vector, search/new/mod.rs:419-508: Asc/Desc criteria and the `sort`
         // list) are not built: such queries are refused one by one rather than answered in plain vector order.  A `sort` list while
         // the criteria lack `sort` is SortRankingRuleMissing (check_sort_criteria, :998-1016), as in keyword searches.
-        if (rc1 == B200_OK) {
-            bool has_sort_criterion = false, has_custom = false;
-            for (int c : hix.settings.criteria) {
-                has_sort_criterion |= c == B200_C_SORT;
-                has_custom |= (c & 0x30000) != 0;
-            }
+        if (rc1 == B200_OK)
             for (uint32_t q = 0; q < b->n_queries; q++) {
-                const bool has_list = b->sort_begin && b->sort_begin[q + 1] > b->sort_begin[q];
-                int code = 0;
-                if (has_list && !has_sort_criterion) {
-                    code = B200_ERR_INVALID;
-                    last_error = "SortRankingRuleMissing: a sort list was given but the ranking rules do not contain `sort`";
-                } else if (has_list || has_custom) {
-                    code = B200_ERR_UNSUPPORTED;
-                    last_error = "sort rules in a semantic search (sort list or Asc/Desc criteria) are not built";
-                }
+                std::vector<SortRule> unused;
+                const char *why = nullptr;
+                const int code = sort_rules(b, q, true, false, unused, why);
                 if (!code) continue;
+                last_error = why;
                 r->n_hits[q] = 0;
                 if (r->status) r->status[q] = code;
                 if (r->n_candidates) r->n_candidates[q] = 0;
             }
-        }
         return rc1;
     }
     if (b->mode != 2) return fail(B200_ERR_INVALID, "unknown search mode");

@@ -339,8 +339,12 @@ struct NcclId {
 };
 
 struct GraphObj;  // S1: opaque query graph (engine_search.cpp)
-struct S1Job;
 void free_graph(GraphObj *);
+
+struct SortRule {  // one sort ranking rule: a field and its direction
+    uint16_t fid;
+    bool asc;
+};
 
 // The host side of a search is a few dozen threads working on the same per-query state.  On a two-socket host it is ~13 % faster
 // (cfg 3, measured) when all of them sit on the socket the GPU hangs off, so a search call narrows the calling thread's affinity to
@@ -414,20 +418,11 @@ struct Engine {
     size_t arena_bytes = 0;
     uint8_t *scratch = nullptr;
     size_t scratch_bytes = 0;
-    DevBuf<uint8_t> d_step;     // per-step input blob
-    DevBuf<uint32_t> d_results; // per-step results
-    DevBuf<Job> d_queue;
-    DevBuf<uint32_t> d_qcount;   // [0] scatter jobs, [1] surviving paths
-    DevBuf<PathOut> d_pathbuf;
     DevBuf<uint32_t> d_docids_out;  // n_queries x limit
     DevBuf<SortDesc> d_sort_desc;   // sort windows of a batch (sort.cu)
     DevBuf<uint32_t> d_sort_keys, d_sort_info;
     DevBuf<unsigned long long> d_universes;  // the batch's distinct filtered universes (documents_ids & filter), n_words64 words each
     DevBuf<uint32_t> d_rowtab;      // n_queries x n_words64: word -> (tag, row) of the query's current activation (ActDesc::row_tab)
-    uint8_t *h_step = nullptr;      // pinned
-    size_t h_step_cap = 0;
-    uint32_t *h_results = nullptr;  // pinned
-    size_t h_results_cap = 0;
     // lev buffers
     DevBuf<LevTerm> d_lev_terms;
     DevBuf<LevRec> d_lev_recs;
@@ -437,7 +432,6 @@ struct Engine {
     DevBuf<uint32_t> d_vsel_ids, d_vsel_n;
     DevBuf<unsigned long long> d_cand, d_vruns, d_vpartial;
     DevBuf<uint16_t> d_vq16;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     std::vector<cudaEvent_t> ev_pool;  // pairs recorded around kernels, resolved after the step's sync
     struct Timed { int cls; size_t a, b; };
     std::vector<Timed> timed;
@@ -478,7 +472,8 @@ struct Engine {
     int search_batch(const b200_query_batch *b, b200_results *r);
     int union_postings(int db, const uint32_t *key_index, uint32_t n_keys, const uint64_t *universe, uint64_t n_universe_words, uint64_t *out);
     DevBuf<uint8_t> d_s2;  // S2 scratch: universe | column | ActDesc | jobs | counters
-    int keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t offset, uint32_t limit, int scoring, S1Job *s1 = nullptr);
+    int keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t offset, uint32_t limit, int scoring);
+    int sort_rules(const b200_query_batch *b, uint32_t qi, bool semantic, bool placeholder, std::vector<SortRule> &out, const char *&why) const;
     // S1 (RankingRule seam): see include/b200milli.h
     int graph_from_tokens(const b200_query_batch *one_query, GraphObj **out);
     struct RuleRun;

@@ -46,14 +46,17 @@ struct WordRef {
     bool derived;
 };
 
-struct QCtx {
-    const HostIndex &ix;
+// the terms of a query; QCtx binds them to the index they come from
+struct QTerms {
     std::vector<ETerm> terms;
     std::vector<EPhrase> phrases;
     std::map<std::vector<int32_t>, uint32_t> phrase_ids;
     std::vector<uint32_t> neg_words;    // dictionary ranks of `-word` tokens (absent words exclude nothing)
     std::vector<uint32_t> neg_phrases;  // phrase ids of `-"..."`
     std::vector<uint16_t> freq_weight;  // TermsMatchingStrategy::Frequency: removal weight per term id (query_graph.rs:303-344)
+};
+struct QCtx : QTerms {
+    const HostIndex &ix;
     explicit QCtx(const HostIndex &i) : ix(i) {}
     uint32_t intern_phrase(const EPhrase &p) {
         auto it = phrase_ids.find(p.words);
@@ -307,7 +310,6 @@ std::vector<std::vector<uint16_t>> removal_order(const QCtx &c, const EGraph &g,
     if (!mandatory && !res.empty()) res.pop_back();
     return res;
 }
-std::vector<std::vector<uint16_t>> removal_order_last(const QCtx &c, const EGraph &g) { return removal_order(c, g, B200_TMS_LAST); }
 
 // ------------------------------------------------------------------------------------------------ activations
 struct ECond {
@@ -325,25 +327,6 @@ struct ECond {
     bool has_start = false;
     ELocated start_subset, end_subset;
     uint16_t col = 0;
-    std::string key() const {
-        std::string s;
-        s.reserve(96);
-        s.push_back((char)rule);
-        term.key(s);
-        s.push_back((char)nbr_typos);
-        s.push_back(prox_uninit ? 'U' : 'T');
-        if (prox_uninit) {
-            left.key(s);
-            s.push_back((char)cost);
-        }
-        s.push_back(has_fid ? 'f' : '-');
-        if (has_fid) s.append(reinterpret_cast<const char *>(&fid), 2);
-        uint32_t np = (uint32_t)positions.size();
-        s.append(reinterpret_cast<const char *>(&np), 4);
-        if (np) s.append(reinterpret_cast<const char *>(positions.data()), positions.size() * 2);
-        s.push_back(exact_in_attribute ? 'E' : 'A');
-        return s;
-    }
 };
 
 struct EEdge {
@@ -402,10 +385,6 @@ struct Level {
     uint64_t universe_count = 0;
 };
 
-struct EmitReq {
-    EmitDesc d;
-};
-
 // Tree mode (no deadline): every needed bucket of a level is expanded as soon as the level's counts are known — the result window of
 // each bucket follows from the counts of the buckets before it, so sibling subtrees are independent searches.  A Node is one rule
 // level of one query: its Level, where it stands in the result order and the scores its documents carry on entry.
@@ -418,14 +397,24 @@ struct Node {
     std::vector<EScore> scores;   // ranking-rule scores on entry (the path of buckets that led here)
 };
 
+// The universe of an activation (ActDesc::p_*): bucket column `col` of its parent level, or the query's universe for its first
+// activation.  cap bounds the activation's rows.
+struct ParentRef {
+    const uint32_t *uw = nullptr;
+    const unsigned long long *ub = nullptr, *out = nullptr;
+    uint32_t rows = 0, ld = 0, col = 0, cap = 0;
+    static ParentRef bucket(const Level &L, uint32_t ci, uint64_t cnt) {
+        return ParentRef{L.uw, L.ub, L.out, L.rows, L.ld, ci, (uint32_t)std::min<uint64_t>(cnt, L.rows)};
+    }
+    static ParentRef universe(const unsigned long long *ub, uint32_t n_words64) { return ParentRef{nullptr, ub, nullptr, n_words64, n_words64, 0, n_words64}; }
+};
+
 // One requested activation: the level it evaluates, the device work description and where its parent universe is.
 struct Pending {
     Level *L = nullptr;           // in QState::levels (sequential mode: stable until the activation completes) or in a Node
     Node *node = nullptr;         // tree mode
     StepOut o;
-    const uint32_t *p_uw = nullptr;
-    const unsigned long long *p_ub = nullptr, *p_out = nullptr;
-    uint32_t p_rows = 0, p_ld = 0, p_col = 0, p_cap = 0;
+    ParentRef parent;
     uint32_t need = 1;            // documents bucket_sort can still use from this activation (ActDesc::need)
     uint32_t tab_shift = 0;       // path de-duplication table = 4096 << tab_shift slots
     size_t demand = 0;            // device bytes asked for (capacity diagnostics)
@@ -434,7 +423,7 @@ struct Pending {
 // What the completion of one activation adds to its query in tree mode.  Activations of the same query complete on different
 // threads; each fills its own ActOut and the query folds them in afterwards (one thread per query).
 struct ActOut {
-    std::vector<EmitReq> emits;
+    std::vector<EmitDesc> emits;
     std::vector<std::unique_ptr<Node>> nodes;
     std::vector<std::unique_ptr<Pending>> pendings;
     std::vector<std::pair<size_t, size_t>> freed;
@@ -459,24 +448,20 @@ struct QState {
     std::vector<std::vector<EScore>> scores;  // per hit
     // device work requested for the next steps (sequential mode: at most one)
     std::vector<std::unique_ptr<Pending>> pendings;
-    std::vector<EmitReq> emits;
+    std::vector<EmitDesc> emits;
     // tree mode
     bool tree = false;
     std::vector<std::unique_ptr<Node>> nodes;
     uint32_t outstanding = 0;  // activations requested and not yet expanded
     const unsigned long long *d_univ = nullptr;  // filtered_universe of the query on the device (nullptr = documents_ids)
     uint64_t univ_count = 0;
-    bool degraded = false, used_negative = false, below_seen = false;
+    bool degraded = false, used_negative = false;
     long polls = 0;                   // Deadline::exceeded() calls so far (stop_after hook)
     const unsigned long long *cand_src = nullptr;  // device bitmap to copy into b200_results::candidates at the lane's next step
     std::vector<uint64_t> term_freq;  // Frequency: documents per term id, filled one device step per term before anything else
     uint32_t n_term_ids = 0;
     // Sort rules of a placeholder search (search/new/mod.rs:351-416): fid and direction per rule; sort_lo/hi: the ranks of the
     // universe the result window holds, produced by sort_window_kernel after the step loop
-    struct SortRule {
-        uint16_t fid;
-        bool asc;
-    };
     std::vector<SortRule> sort_rules;
     bool sort_pending = false;
     uint32_t sort_lo = 0, sort_hi = 0;
@@ -980,8 +965,6 @@ void finish_state_graph(Level &L, const std::vector<AE> &aedges, uint32_t root, 
     if (L.sedges.size() > 60000) throw TooComplex{"ranking-rule graph too large"};
     L.want_paths = want_paths;
 }
-
-constexpr size_t MAX_PATHS = 60000;
 
 // Build graph + enumerate all START->END paths (cheapest_paths.rs semantics without the dead-end cache: every
 // path is handed to the device, which finds the empty ones itself).
@@ -1695,208 +1678,204 @@ double global_score_of(const std::vector<EScore> &sc) {
     return (double)rk / (double)mx;
 }
 
-struct Blob {  // step input blob with aligned sections
-    std::vector<uint8_t> bytes;
-    template <class T>
-    size_t add(const std::vector<T> &v) {
-        size_t off = (bytes.size() + 15) & ~(size_t)15;
-        bytes.resize(off + v.size() * sizeof(T));
-        if (!v.empty()) memcpy(bytes.data() + off, v.data(), v.size() * sizeof(T));
-        return off;
-    }
-};
-
 }  // namespace
 
-// S1: an opaque query graph (QueryGraph + the terms it refers to) and the job description keyword_batch runs for the seam
+// S1: an opaque query graph (QueryGraph + the terms it refers to)
 struct GraphObj {
     QCtx ctx;
     EGraph graph;
-    explicit GraphObj(const HostIndex &ix) : ctx(ix) {}
+    GraphObj(const QCtx &c, const EGraph &g) : ctx(c), graph(g) {}
 };
-struct S1Job {
-    enum { GRAPH_FROM_TOKENS, RULE } mode = GRAPH_FROM_TOKENS;
-    // GRAPH_FROM_TOKENS: out
-    GraphObj *graph_out = nullptr;
-    // RULE: in
-    const GraphObj *graph_in = nullptr;
-    int rule_kind = 0;  // RuleKind
-    // RULE: out, one entry per cost of the rule in ascending cost order (empty buckets included)
-    struct Bucket {
-        uint32_t rank, max_rank;
-        uint64_t count;
-        std::vector<uint64_t> bitmap;  // dense, n_words64 words
-        GraphObj *child = nullptr;     // the query graph of the paths that produced the bucket (nullptr: no path information)
-    };
-    std::vector<Bucket> buckets;
+// S1: one bucket of the rule rule_start ran, in ascending cost order (empty buckets included)
+struct RuleBucket {
+    uint32_t rank, max_rank;
+    uint64_t count;
+    std::vector<uint64_t> bitmap;  // dense, n_words64 words
+    GraphObj *child = nullptr;     // the query graph of the paths that produced the bucket (nullptr: no path information)
 };
 
 namespace {
 
-template <class F>
-void parallel_for(size_t n, unsigned nt, F f) {
-    if (n == 0) return;
-    nt = (unsigned)std::min<size_t>(nt, n);
-    if (nt <= 1) {
-        for (size_t i = 0; i < n; i++) f(i);
-        return;
-    }
-    std::atomic<size_t> next{0};
-    std::vector<std::thread> th;
-    for (unsigned t = 0; t < nt; t++)
-        th.emplace_back([&]() {
-            for (;;) {
-                size_t i = next.fetch_add(1);
-                if (i >= n) break;
-                f(i);
-            }
-        });
-    for (auto &x : th) x.join();
+// worker threads of the host phases (B200_HOST_THREADS; the calling thread counts as one)
+unsigned host_threads() {
+    unsigned hw = std::thread::hardware_concurrency();
+    const char *env = getenv("B200_HOST_THREADS");
+    return env ? (unsigned)atoi(env) : std::max(4u, std::min(32u, hw / 2));
 }
 
-}  // namespace
+// An activation waiting in a lane: its query and its request
+struct Cand {
+    uint32_t qi;
+    Pending *pd;
+};
+// Where pass 1 placed one scheduled activation: its offsets in every section of the step blob, its device memory and its row table
+struct Plan {
+    uint32_t jobs, sets, words, colprog, states, edges, costs, tiles, probes, res_off, ctiles, n_seg, prog;
+    uint32_t ld, cls, tab_size, rpt, rt_slot, rt_tag;
+    uint8_t *pb;
+    size_t coff, toff, soff_from_end;
+    bool identity;
+};
+// One step of a lane: what joins it (pass 1), the totals that size its blob and where the blob's sections start (pass 2)
+struct Step {
+    std::vector<uint32_t> emit_q;
+    std::vector<Cand> cand_q;
+    std::vector<Plan> plan;
+    std::vector<size_t> sched;  // indices in cand_q of the activations that join this step
+    uint32_t n_jobs = 0, n_sets = 0, n_words = 0, n_colprog = 0, n_states = 0, n_edges = 0, n_costs_tot = 0, n_tiles = 0, n_probes = 0, res_words = 0, n_prog = 0;
+    uint32_t n_ctiles = 0, n_tiles_cls[EVAL_CLASSES + 1] = {};
+    bool want_paths_cls[EVAL_CLASSES + 1] = {};
+    bool multi_segment = false;
+    size_t z_used = 0, s_used = 0;
+    uint64_t compact_bytes = 0, eval_bytes = 0, fill_bytes = 0;
+    uint32_t tile_base[EVAL_CLASSES + 2] = {};
+    uint32_t n_emits = 0;
+    size_t o_acts = 0, o_sets = 0, o_words = 0, o_colprog = 0, o_states = 0, o_edges = 0, o_costs = 0, o_prog = 0, o_tiles = 0, o_ctiles = 0, o_emits = 0,
+           o_jobs = 0, o_nstatic = 0, nbytes = 0;
+};
+// B200_WORK_HIST=1: where the steps' work comes from (developer statistics, see tools/)
+struct WorkHist {
+    std::mutex mu;
+    uint64_t lists[4][33][2] = {};  // [universe class][log2 card | 32 = dense] -> {lists, stored bytes}
+    uint64_t eval[10][4][4] = {};   // [rule kind][universe class] -> {activations, rows(ld), rows x program ops, rows x columns}
+    uint64_t probes[4] = {};
+};
 
-// ================================================================================================ driver
-int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t offset, uint32_t limit, int scoring, S1Job *s1) {
-    CU(cudaSetDevice(device), "cudaSetDevice");
-    AffinityScope on_gpu_socket(affinity);  // before any thread of this call is created
-    const uint32_t NQ = b->n_queries;
-    if (!pool) {
-        unsigned hw = std::thread::hardware_concurrency();
-        const char *env = getenv("B200_HOST_THREADS");
-        unsigned nt = env ? (unsigned)atoi(env) : std::max(4u, std::min(32u, hw / 2));
-        pool.reset(new WorkerPool(std::max(1u, nt) - 1));  // the calling thread works too
-    }
-    auto pfor = [&](size_t n, std::function<void(size_t)> f) { pool->run(n, std::move(f)); };
+// One keyword_batch call: the batch, its per-query state and the lanes that step it.  The phases are member functions; the lanes'
+// driver threads run launch() / finish() concurrently, each on its own lanes and queries.
+struct KeywordBatch {
     using clk = std::chrono::steady_clock;
-    auto ms_since = [](clk::time_point t) { return std::chrono::duration<double, std::milli>(clk::now() - t).count(); };
-    auto t_total = clk::now();
-    const bool skip_scoring = scoring == 0;
-    const uint32_t length = limit, from = offset;
-    const int tms = b->terms_matching_strategy;
-    std::vector<std::unique_ptr<QState>> qs(NQ);
-    for (uint32_t i = 0; i < NQ; i++) qs[i].reset(new QState(hix));
+    Engine &eng;
+    const HostIndex &hix;
+    const DeviceIndex &dix;
+    b200_stats &stats;
+    Lane *const lanes;
+    const b200_query_batch *b;
+    b200_results *r;
+    const clk::time_point t_total = clk::now();
+    const uint32_t NQ, from, length;
+    const int tms;
+    const bool skip_scoring;
+    const bool has_thr;
+    const double thr;
+    const bool has_budget;
+    const clk::time_point deadline_at;
+    const long stop_after;
+    std::vector<std::unique_ptr<QState>> qs;
+    const std::vector<int> rules;
+    // tree-parallel bucket sort unless the order of bucket requests is observable: a deadline polls once per request, and a bucket
+    // dropped by the ranking-score threshold moves every later hit forward
+    const bool use_tree;
+    // rule_start: the buckets of its single activation are collected here instead of being sorted further
+    std::vector<RuleBucket> *rule_buckets = nullptr;
+    unsigned n_drivers = 1, lanes_per_driver = 1, n_lanes = 1;
+    std::vector<std::vector<std::unique_ptr<Pending>>> lane_acts;  // per lane: the activations of its step in flight
+    bool use_rowtab = false;
+    std::vector<uint32_t> slot_tag;
+    const uint32_t rowtab_min_rows = getenv("B200_ROWTAB_MIN") ? (uint32_t)atoi(getenv("B200_ROWTAB_MIN")) : 64;
+    const uint32_t eval_rpt_big = getenv("B200_EVAL_RPT") ? (uint32_t)std::max(1, std::min(8, atoi(getenv("B200_EVAL_RPT")))) : 4;
+    static constexpr size_t PATH_CAP = (size_t)1 << 20;
+    const std::unique_ptr<WorkHist> work_hist{getenv("B200_WORK_HIST") ? new WorkHist() : nullptr};
+    // optional host profile (B200_PROFILE=1): summed thread time per section, printed per batch
+    enum ProfSection { PROF_PATHS, PROF_GRAPH_RULE, PROF_REQUEST, PROF_ADVANCE, PROF_SECTIONS };
+    const bool prof = getenv("B200_PROFILE") != nullptr;
+    std::atomic<uint64_t> prof_ns[PROF_SECTIONS] = {};
+    struct ProfScope {
+        std::atomic<uint64_t> *slot;
+        clk::time_point t0;
+        explicit ProfScope(std::atomic<uint64_t> *s) : slot(s) {
+            if (slot) t0 = clk::now();
+        }
+        ProfScope(const ProfScope &) = delete;
+        ~ProfScope() {
+            if (slot) *slot += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(clk::now() - t0).count();
+        }
+    };
+    ProfScope profile(ProfSection s) { return ProfScope(prof ? &prof_ns[s] : nullptr); }
+
+    KeywordBatch(Engine &e, const b200_query_batch *batch, b200_results *res, uint32_t offset, uint32_t limit, int scoring)
+        : eng(e), hix(e.hix), dix(e.dix), stats(e.stats), lanes(e.lanes), b(batch), r(res), NQ(batch->n_queries), from(offset), length(limit),
+          tms(batch->terms_matching_strategy), skip_scoring(scoring == 0), has_thr(batch->has_ranking_score_threshold != 0),
+          thr(batch->ranking_score_threshold), has_budget(batch->time_budget_ns > 0), deadline_at(t_total + std::chrono::nanoseconds(batch->time_budget_ns)),
+          stop_after((long)batch->stop_after), qs(batch->n_queries), rules(rule_list(e.hix.settings, batch->terms_matching_strategy)),
+          use_tree(stop_after < 0 && !has_budget && !has_thr && !getenv("B200_NO_TREE")) {
+        if (!eng.pool) eng.pool.reset(new WorkerPool(std::max(1u, host_threads()) - 1));  // the calling thread works too
+        for (uint32_t i = 0; i < NQ; i++) qs[i].reset(new QState(hix));
+    }
+    int fail(int code, const std::string &msg) { return eng.fail(code, msg); }
+    int cuda_fail(cudaError_t e, const char *what) { return eng.cuda_fail(e, what); }
+    static double ms_since(clk::time_point t) { return std::chrono::duration<double, std::milli>(clk::now() - t).count(); }
+    void pfor(size_t n, std::function<void(size_t)> f) { eng.pool->run(n, std::move(f)); }
+    // filtered_universe of a query on the device
+    const unsigned long long *universe_of(const QState &q) const { return q.d_univ ? q.d_univ : dix.base_ub; }
+    // contiguous query ranges per lane, so that the first half of the drivers can start while the second half's terms are derived
+    uint32_t lane_lo(unsigned l) const { return (uint32_t)((uint64_t)NQ * l / n_lanes); }
 
     // ---- phase 1: tokens -> terms -> query graph
-    auto t_ph = clk::now();
-    if (s1 && s1->mode == S1Job::RULE) {
-        QState &q = *qs[0];
-        q.ctx.terms = s1->graph_in->ctx.terms;
-        q.ctx.phrases = s1->graph_in->ctx.phrases;
-        q.ctx.phrase_ids = s1->graph_in->ctx.phrase_ids;
-        q.ctx.neg_words = s1->graph_in->ctx.neg_words;
-        q.ctx.neg_phrases = s1->graph_in->ctx.neg_phrases;
-        q.ctx.freq_weight = s1->graph_in->ctx.freq_weight;
-        q.graph = s1->graph_in->graph;
-    } else
-    pfor(NQ, [&](size_t i) {
-        QState &q = *qs[i];
-        try {
-            parse_query(q, b, (uint32_t)i);
-        } catch (const UnsupportedQuery &u) {
-            q.status = B200_ERR_UNSUPPORTED;
-            q.error = u.why;
-            q.done = true;
-        }
-    });
-    stats.host_ms[0] += ms_since(t_ph);
-    // ---- sort rules (search/new/mod.rs:351-416, 651-716): the `Sort` criterion expands to the query's `sort` list at its position,
-    // once; Asc(f) / Desc(f) criteria add one rule each; a field sorted earlier in the list is skipped
-    {
-        bool has_sort_criterion = false, has_custom = false;
-        for (int c : hix.settings.criteria) {
-            has_sort_criterion |= c == B200_C_SORT;
-            has_custom |= (c & 0x30000) != 0;
-        }
-        if (b->sort_begin || has_custom)
-            for (uint32_t i = 0; i < NQ; i++) {
-                QState &q = *qs[i];
-                if (q.done) continue;
-                const uint32_t s0 = b->sort_begin ? b->sort_begin[i] : 0, s1_ = b->sort_begin ? b->sort_begin[i + 1] : 0;
-                auto refuse = [&](int code, const char *why) {
-                    q.status = code;
-                    q.error = why;
-                    q.done = true;
-                };
-                if (s1_ > s0 && !has_sort_criterion) {  // check_sort_criteria (search/new/mod.rs:998-1016)
-                    refuse(B200_ERR_INVALID, "SortRankingRuleMissing: a sort list was given but the ranking rules do not contain `sort`");
-                    continue;
-                }
-                if (s1_ > s0 && (!b->sort_fid || !b->sort_asc)) {
-                    refuse(B200_ERR_INVALID, "sort_begin without sort_fid / sort_asc");
-                    continue;
-                }
-                std::vector<QState::SortRule> sr;
-                std::vector<uint16_t> sorted;
-                bool sort_done = false;
-                auto add = [&](uint16_t fid, bool asc) {
-                    // 0xFFFF stands for every field absent from the fields map: its entries are never "already sorted" (the caller,
-                    // which sees the names, drops a repeated absent name)
-                    if (fid != 0xFFFF && std::find(sorted.begin(), sorted.end(), fid) != sorted.end()) return;
-                    sorted.push_back(fid);
-                    sr.push_back(QState::SortRule{fid, asc});
-                };
-                for (int c : hix.settings.criteria) {
-                    if (c == B200_C_SORT && !sort_done) {
-                        sort_done = true;
-                        for (uint32_t k = s0; k < s1_; k++) add(b->sort_fid[k], b->sort_asc[k] != 0);
-                    } else if (c & 0x10000)
-                        add((uint16_t)(c & 0xffff), true);
-                    else if (c & 0x20000)
-                        add((uint16_t)(c & 0xffff), false);
-                }
-                if (sr.empty()) continue;
-                if (b->mode != 0)
-                    refuse(B200_ERR_UNSUPPORTED, "sort in a semantic or hybrid search (needs the ScoreValue::Sort comparator of hybrid.rs)");
-                else if (!q.placeholder)
-                    refuse(B200_ERR_UNSUPPORTED, "sort rule in a search with query terms (sort is built for placeholder searches)");
-                else if (sr.size() > B200_MAX_SCORES)
-                    refuse(B200_ERR_UNSUPPORTED, "more than B200_MAX_SCORES sort rules");
-                else if (b->stop_after >= 0)
-                    refuse(B200_ERR_UNSUPPORTED, "stop_after together with a sort rule (the sort window is one device step; its polls are not counted)");
-                else
-                    q.sort_rules = std::move(sr);
+    void parse() {
+        auto t_ph = clk::now();
+        pfor(NQ, [&](size_t i) {
+            QState &q = *qs[i];
+            try {
+                parse_query(q, b, (uint32_t)i);
+            } catch (const UnsupportedQuery &u) {
+                q.status = B200_ERR_UNSUPPORTED;
+                q.error = u.why;
+                q.done = true;
             }
+        });
+        stats.host_ms[0] += ms_since(t_ph);
+    }
+    void resolve_sort_rules() {
+        for (uint32_t i = 0; i < NQ; i++) {
+            QState &q = *qs[i];
+            if (q.done) continue;
+            const char *why = nullptr;
+            const int code = eng.sort_rules(b, i, false, q.placeholder, q.sort_rules, why);
+            if (code != B200_OK) {
+                q.status = code;
+                q.error = why;
+                q.done = true;
+            }
+        }
     }
     // ---- filtered universes (search/new/mod.rs:719): every distinct bitmap is intersected with documents_ids and uploaded once
-    const bool has_thr = b->has_ranking_score_threshold != 0;
-    const double thr = b->ranking_score_threshold;
-    const bool has_budget = b->time_budget_ns > 0;
-    const auto deadline_at = t_total + std::chrono::nanoseconds(b->time_budget_ns);
-    const long stop_after = (long)b->stop_after;
-    if (r->candidates && has_thr) return fail(B200_ERR_UNSUPPORTED, "candidates bitmap together with a ranking-score threshold");
-    if (r->candidates && r->candidates_words < hix.n_words64) return fail(B200_ERR_INVALID, "candidates_words smaller than the document range");
-    if (b->universes) {
-        const uint64_t W = hix.n_words64;
-        if (b->n_universe_words < W) return fail(B200_ERR_INVALID, "universe bitmaps shorter than the document range");
-        std::map<const uint64_t *, uint32_t> slot_of;
-        for (uint32_t i = 0; i < NQ; i++)
-            if (b->universes[i]) slot_of.emplace(b->universes[i], 0);
-        uint32_t ns = 0;
-        for (auto &kv : slot_of) kv.second = ns++;
-        CU(d_universes.reserve((size_t)std::max(1u, ns) * W), "alloc universes");
-        std::vector<uint64_t> counts(ns, 0), tmp(W);
-        for (auto &kv : slot_of) {
-            uint64_t c = 0;
-            for (uint64_t w = 0; w < W; w++) {
-                tmp[w] = kv.first[w] & hix.base_ub[w];
-                c += (uint64_t)__builtin_popcountll(tmp[w]);
+    int stage_universes() {
+        if (r->candidates && has_thr) return fail(B200_ERR_UNSUPPORTED, "candidates bitmap together with a ranking-score threshold");
+        if (r->candidates && r->candidates_words < hix.n_words64) return fail(B200_ERR_INVALID, "candidates_words smaller than the document range");
+        if (b->universes) {
+            const uint64_t W = hix.n_words64;
+            if (b->n_universe_words < W) return fail(B200_ERR_INVALID, "universe bitmaps shorter than the document range");
+            std::map<const uint64_t *, uint32_t> slot_of;
+            for (uint32_t i = 0; i < NQ; i++)
+                if (b->universes[i]) slot_of.emplace(b->universes[i], 0);
+            uint32_t ns = 0;
+            for (auto &kv : slot_of) kv.second = ns++;
+            CU(eng.d_universes.reserve((size_t)std::max(1u, ns) * W), "alloc universes");
+            std::vector<uint64_t> counts(ns, 0), tmp(W);
+            for (auto &kv : slot_of) {
+                uint64_t c = 0;
+                for (uint64_t w = 0; w < W; w++) {
+                    tmp[w] = kv.first[w] & hix.base_ub[w];
+                    c += (uint64_t)__builtin_popcountll(tmp[w]);
+                }
+                counts[kv.second] = c;
+                CU(cudaMemcpy(eng.d_universes.p + (size_t)kv.second * W, tmp.data(), W * 8, cudaMemcpyHostToDevice), "H2D universe");
+                stats.h2d_bytes += W * 8;
             }
-            counts[kv.second] = c;
-            CU(cudaMemcpy(d_universes.p + (size_t)kv.second * W, tmp.data(), W * 8, cudaMemcpyHostToDevice), "H2D universe");
-            stats.h2d_bytes += W * 8;
+            for (uint32_t i = 0; i < NQ; i++)
+                if (b->universes[i]) {
+                    uint32_t sl = slot_of[b->universes[i]];
+                    qs[i]->d_univ = eng.d_universes.p + (size_t)sl * W;
+                    qs[i]->univ_count = counts[sl];
+                }
         }
         for (uint32_t i = 0; i < NQ; i++)
-            if (b->universes[i]) {
-                uint32_t sl = slot_of[b->universes[i]];
-                qs[i]->d_univ = d_universes.p + (size_t)sl * W;
-                qs[i]->univ_count = counts[sl];
-            }
+            if (!qs[i]->d_univ) qs[i]->univ_count = hix.n_documents;
+        return B200_OK;
     }
-    for (uint32_t i = 0; i < NQ; i++)
-        if (!qs[i]->d_univ) qs[i]->univ_count = hix.n_documents;
-    // ---- phase 2 (per wave, see below): typo derivations for every term of queries [lo, hi) in one device sweep
-    auto derive_range = [&](uint32_t lo, uint32_t hi) -> int {
+    // ---- phase 2 (per wave, see drive_waves): typo derivations for every term of queries [lo, hi) in one device sweep
+    int derive_range(uint32_t lo, uint32_t hi) {
         auto t_ph = clk::now();
         std::vector<char> wbytes;
         std::vector<uint32_t> woff{0};
@@ -1933,7 +1912,7 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         uint32_t n = (uint32_t)mt.size();
         std::vector<uint32_t> one((size_t)n * 150), n_one(n), two((size_t)n * 50), n_two(n);
         if (n) {
-            int rc = derive_batch(n, wbytes.data(), woff.data(), mt.data(), ip.data(), one.data(), n_one.data(), two.data(), n_two.data());
+            int rc = eng.derive_batch(n, wbytes.data(), woff.data(), mt.data(), ip.data(), one.data(), n_one.data(), two.data(), n_two.data());
             if (rc != B200_OK) return rc;
         }
         stats.host_ms[1] += ms_since(t_ph);
@@ -1953,33 +1932,11 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         });
         stats.host_ms[2] += ms_since(t_ph);
         return B200_OK;
-    };
-    // ---- result buffers
-    CU(d_docids_out.reserve((size_t)NQ * std::max(1u, length)), "alloc results");
-    // optional host profile (B200_PROFILE=1): summed thread time per section, printed per batch
-    static std::atomic<uint64_t> prof_ns[8];
-    const bool prof = getenv("B200_PROFILE") != nullptr;
-    if (prof)
-        for (auto &x : prof_ns) x = 0;
-    struct ProfScope {
-        std::atomic<uint64_t> *slot;
-        clk::time_point t0;
-        ProfScope(std::atomic<uint64_t> *s2) : slot(s2) {
-            if (slot) t0 = clk::now();
-        }
-        ~ProfScope() {
-            if (slot) *slot += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(clk::now() - t0).count();
-        }
-    };
-#define PROF(i) ProfScope prof_scope_##i(prof ? &prof_ns[i] : nullptr)
+    }
+
     // ---- phase 3: initial requests (universe resolution) or placeholder emission
-    std::vector<int> rules = rule_list(hix.settings, tms);
-    // tree-parallel bucket sort unless the order of bucket requests is observable: a deadline polls once per request, and a bucket
-    // dropped by the ranking-score threshold moves every later hit forward
-    const bool use_tree = stop_after < 0 && !has_budget && !has_thr && !getenv("B200_NO_TREE");
-    auto make_pending = [&](QState &q, Level &L, const uint32_t *p_uw, const unsigned long long *p_ub, const unsigned long long *p_out, uint32_t p_rows,
-                            uint32_t p_ld, uint32_t p_col, uint32_t cap, uint64_t off0, std::vector<std::unique_ptr<Pending>> &dst) -> Pending * {
-        PROF(2);
+    Pending *make_pending(QState &q, Level &L, const ParentRef &parent, uint64_t off0, std::vector<std::unique_ptr<Pending>> &dst) {
+        ProfScope ps = profile(PROF_REQUEST);
         std::unique_ptr<Pending> pd(new Pending());
         if (L.kind == RK_EXACT_ATTRIBUTE) prepare_exact_attribute(q.ctx, L, pd->o);
         emit_activation_work(q.ctx, L, pd->o);
@@ -1988,35 +1945,26 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         const uint64_t window_end = (uint64_t)from + length;
         pd->need = (uint32_t)std::min<uint64_t>(0xffffffffull, window_end > off0 ? window_end - off0 : 1);
         if (pd->need == 0) pd->need = 1;
-        pd->p_uw = p_uw;
-        pd->p_ub = p_ub;
-        pd->p_out = p_out;
-        pd->p_rows = p_rows;
-        pd->p_ld = p_ld;
-        pd->p_col = p_col;
-        pd->p_cap = cap;
+        pd->parent = parent;
         dst.push_back(std::move(pd));
         return dst.back().get();
-    };
+    }
     // sequential mode: the level goes on the query's stack
-    auto request_activation = [&](QState &q, Level &&L, const uint32_t *p_uw, const unsigned long long *p_ub, const unsigned long long *p_out,
-                                  uint32_t p_rows, uint32_t p_ld, uint32_t p_col, uint32_t cap) -> Pending * {
+    Pending *request_activation(QState &q, Level &&L, const ParentRef &parent) {
         q.levels.push_back(std::move(L));
         // documents already returned or skipped: everything before this level in result order
-        Pending *pd = make_pending(q, q.levels.back(), p_uw, p_ub, p_out, p_rows, p_ld, p_col, cap, q.cur_offset, q.pendings);
+        Pending *pd = make_pending(q, q.levels.back(), parent, q.cur_offset, q.pendings);
         pd->L = &q.levels.back();
         return pd;
-    };
-    // tree mode: the level becomes a node under `parent`
-    auto request_node = [&](QState &q, Node *parent, Level &&L, const uint32_t *p_uw, const unsigned long long *p_ub, const unsigned long long *p_out,
-                            uint32_t p_rows, uint32_t p_ld, uint32_t p_col, uint32_t cap, uint64_t off0, std::vector<EScore> scores,
-                            ActOut *out) -> Pending * {
+    }
+    // tree mode: the level becomes a node under `parent_node`
+    Pending *request_node(QState &q, Node *parent_node, Level &&L, const ParentRef &parent, uint64_t off0, std::vector<EScore> scores, ActOut *out) {
         std::unique_ptr<Node> nd(new Node());
         nd->L = std::move(L);
-        nd->parent = parent;
+        nd->parent = parent_node;
         nd->off0 = off0;
         nd->scores = std::move(scores);
-        if (parent) parent->live_children++;
+        if (parent_node) parent_node->live_children++;
         Node *np = nd.get();
         if (out)
             out->nodes.push_back(std::move(nd));  // the query counts it when it folds `out` in
@@ -2024,13 +1972,66 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             q.outstanding++;
             q.nodes.push_back(std::move(nd));
         }
-        Pending *pd = make_pending(q, np->L, p_uw, p_ub, p_out, p_rows, p_ld, p_col, cap, off0, out ? out->pendings : q.pendings);
+        Pending *pd = make_pending(q, np->L, parent, off0, out ? out->pendings : q.pendings);
         pd->L = &np->L;
         pd->node = np;
         return pd;
-    };
+    }
+    // The Level of ranking rule `kind` at position `rule_idx` over `graph`.  The matching strategy shapes the first rule when it is
+    // Words; nothing descends from a `last` rule, so its buckets are emitted without computing their paths.
+    Level rule_level(const QCtx &ctx, int rule_idx, int kind, EGraph graph, bool last) {
+        Level C;
+        C.rule_idx = rule_idx;
+        C.kind = kind;
+        C.graph = std::move(graph);
+        if (C.kind != RK_EXACT_ATTRIBUTE) {
+            ProfScope ps = profile(PROF_GRAPH_RULE);
+            prepare_graph_rule(ctx, C.kind, rule_idx == 0 && C.kind == RK_WORDS, tms, C);
+        }
+        if (last) C.want_paths = false;
+        return C;
+    }
+    // The query graph of the paths that put documents into bucket `ci` of L, in visiting order (= lexicographic in edge ids): what
+    // the next rule iterates on.  ExactAttribute hands its own graph down.
+    EGraph child_graph(const Level &L, size_t ci) {
+        if (L.kind == RK_EXACT_ATTRIBUTE) return L.graph;
+        ProfScope ps = profile(PROF_PATHS);
+        std::vector<const SurvPath *> sp;
+        for (auto &p : L.surv)
+            if (p.cost_idx == ci) sp.push_back(&p);
+        std::sort(sp.begin(), sp.end(), [](const SurvPath *x, const SurvPath *y) { return x->edges < y->edges; });
+        std::vector<std::vector<const ECond *>> good;
+        for (auto *p : sp) {
+            std::vector<const ECond *> pc;
+            for (auto e : p->edges)
+                if (L.sedges[e].cond >= 0) pc.push_back(&L.conds[L.sedges[e].cond]);
+            good.push_back(std::move(pc));
+        }
+        return build_from_paths(good);
+    }
+    // The documents [skip, skip + take) of bucket columns [col_lo, col_hi) of L — or, without a level, of the query's universe in docid
+    // order — written to offset `at` of the query's result row (the driver turns the offset into a device pointer)
+    EmitDesc emit_desc(const QState &q, const Level *L, uint32_t col_lo, uint32_t col_hi, uint64_t skip, uint64_t take, uint64_t at) const {
+        EmitDesc d{};
+        if (L) {
+            d.uw = L->uw;
+            d.ub = L->ub;
+            d.out = L->out;
+            d.rows = L->rows;
+            d.ld = L->ld;
+        } else {
+            d.ub = universe_of(q);
+            d.rows = d.ld = hix.n_words64;
+        }
+        d.col_lo = col_lo;
+        d.col_hi = col_hi;
+        d.skip = (uint32_t)skip;
+        d.take = (uint32_t)take;
+        d.dst = reinterpret_cast<uint32_t *>((uintptr_t)at);
+        return d;
+    }
     // resolve_maximally_reduced_query_graph (search/new/mod.rs:273-301)
-    auto start_resolve = [&](QState &q) {
+    void start_resolve(QState &q) {
         Level L;
         L.kind = RK_RESOLVE;
         L.graph = q.graph;
@@ -2041,14 +2042,15 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             remove_nodes_keep_edges(L.graph, rm);
         }
         prepare_resolve(q.ctx, L);
+        const ParentRef univ = ParentRef::universe(universe_of(q), hix.n_words64);
         if (q.tree)
-            request_node(q, nullptr, std::move(L), nullptr, q.d_univ ? q.d_univ : dix.base_ub, nullptr, hix.n_words64, hix.n_words64, 0, hix.n_words64, 0, {}, nullptr);
+            request_node(q, nullptr, std::move(L), univ, 0, {}, nullptr);
         else
-            request_activation(q, std::move(L), nullptr, q.d_univ ? q.d_univ : dix.base_ub, nullptr, hix.n_words64, hix.n_words64, 0, hix.n_words64);
-    };
+            request_activation(q, std::move(L), univ);
+    }
     // Frequency (query_graph.rs:303-344): documents of term id t = union of the docids of every node covering t, counted over the
     // whole index — one resolve-shaped activation START -> {covering nodes} -> END per term id
-    auto start_freq = [&](QState &q, uint32_t t) {
+    void start_freq(QState &q, uint32_t t) {
         Level L;
         L.kind = RK_FREQ;
         L.rule_idx = (int)t;
@@ -2071,23 +2073,12 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                 sorted_insert(g.nodes[1].pred, id);
             }
         prepare_resolve(q.ctx, L);
-        request_activation(q, std::move(L), nullptr, dix.base_ub, nullptr, hix.n_words64, hix.n_words64, 0, hix.n_words64);
-    };
-    auto start_query = [&](QState &q) {
+        request_activation(q, std::move(L), ParentRef::universe(dix.base_ub, hix.n_words64));
+    }
+    void start_query(QState &q) {
         q.rules = rules;
-        // tree mode unless a deadline is in force (its polls are defined on the sequential order of bucket requests) or S1 drives one rule
-        q.tree = use_tree && !s1;
-        if (s1 && s1->mode == S1Job::RULE) {
-            // S1: one ranking rule over the caller's universe and query graph (RankingRule::start_iteration)
-            Level C;
-            C.rule_idx = 0;
-            C.kind = s1->rule_kind;
-            C.graph = q.graph;
-            if (C.kind != RK_EXACT_ATTRIBUTE) prepare_graph_rule(q.ctx, C.kind, C.kind == RK_WORDS, tms, C);
-            Pending *pd = request_activation(q, std::move(C), nullptr, q.d_univ ? q.d_univ : dix.base_ub, nullptr, hix.n_words64, hix.n_words64, 0, hix.n_words64);
-            pd->need = 0xffffffffu;  // every bucket may be asked for: walk them all
-            return;
-        }
+        // tree mode unless a deadline is in force (its polls are defined on the sequential order of bucket requests)
+        q.tree = use_tree;
         if (q.neg_only) {
             q.tree = false;
             Level L;
@@ -2103,7 +2094,7 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             std::vector<AEdge> ae{{0, 1, 0, 0}};  // START -[ignored documents]-> END
             finish_state_graph(L, ae, 0, 1, false);
             L.next_max_cost = 1;
-            request_activation(q, std::move(L), nullptr, q.d_univ ? q.d_univ : dix.base_ub, nullptr, hix.n_words64, hix.n_words64, 0, hix.n_words64);
+            request_activation(q, std::move(L), ParentRef::universe(universe_of(q), hix.n_words64));
             return;
         }
         if (q.placeholder && !q.sort_rules.empty()) {
@@ -2111,22 +2102,14 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             // one sort_window_kernel launch after the step loop.  Deadline::exceeded() is polled before the first bucket request
             // (bucket_sort.rs:206-264): when the budget is already spent the universe is returned as it is, Skipped and degraded.
             q.n_candidates = q.univ_count;
-            q.cand_src = q.d_univ ? q.d_univ : dix.base_ub;
+            q.cand_src = universe_of(q);
             uint64_t avail = q.univ_count > from ? q.univ_count - from : 0;
             uint32_t take = (uint32_t)std::min<uint64_t>(avail, length);
             if (has_budget && clk::now() >= deadline_at) {
                 q.degraded = true;
-                EmitReq e{};
-                e.d.uw = nullptr;
-                e.d.ub = q.d_univ ? q.d_univ : dix.base_ub;
-                e.d.out = nullptr;
-                e.d.rows = hix.n_words64;
-                e.d.ld = hix.n_words64;
-                e.d.skip = from;
-                e.d.take = take;
                 q.n_results = take;
                 q.scores.assign(take, std::vector<EScore>{EScore{B200_S_SKIPPED, 0, 1, -1.f}});
-                if (take) q.emits.push_back(e);
+                if (take) q.emits.push_back(emit_desc(q, nullptr, 0, 0, from, take, 0));
             } else {
                 q.n_results = take;
                 q.scores.assign(take, {});
@@ -2140,19 +2123,12 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         if (q.placeholder) {
             // placeholder search: no text rules (search/new/mod.rs:353-416) -> universe in docid order (bucket_sort.rs:104-116)
             q.n_candidates = q.univ_count;
-            q.cand_src = q.d_univ ? q.d_univ : dix.base_ub;
-            EmitReq e{};
-            e.d.uw = nullptr;
-            e.d.ub = q.d_univ ? q.d_univ : dix.base_ub;
-            e.d.out = nullptr;
-            e.d.rows = hix.n_words64;
-            e.d.ld = hix.n_words64;
-            e.d.skip = from;
+            q.cand_src = universe_of(q);
             uint64_t avail = q.univ_count > from ? q.univ_count - from : 0;
-            e.d.take = (uint32_t)std::min<uint64_t>(avail, length);
-            q.n_results = e.d.take;
+            const uint32_t take = (uint32_t)std::min<uint64_t>(avail, length);
+            q.n_results = take;
             q.scores.assign(q.n_results, {});
-            if (e.d.take) q.emits.push_back(e);
+            if (take) q.emits.push_back(emit_desc(q, nullptr, 0, 0, from, take, 0));
             q.done = true;
             return;
         }
@@ -2167,8 +2143,8 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             }
         }
         start_resolve(q);
-    };
-    auto start_range = [&](uint32_t lo, uint32_t hi) {
+    }
+    void start_range(uint32_t lo, uint32_t hi) {
         auto t_ph = clk::now();
         pfor(hi - lo, [&](size_t i) {
             QState &q = *qs[lo + i];
@@ -2182,9 +2158,43 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             }
         });
         stats.host_ms[5] += ms_since(t_ph);
-    };
+    }
+    // S1: one ranking rule over the caller's universe and query graph (RankingRule::start_iteration); collect_rule_buckets() takes
+    // its result
+    void start_rule(QState &q, int kind) {
+        auto t_ph = clk::now();
+        try {
+            Pending *pd = request_activation(q, rule_level(q.ctx, 0, kind, q.graph, false), ParentRef::universe(universe_of(q), hix.n_words64));
+            pd->need = 0xffffffffu;  // every bucket may be asked for: walk them all
+        } catch (const TooComplex &t) {
+            q.status = B200_ERR_CAPACITY;
+            q.error = t.why;
+            q.done = true;
+        }
+        stats.host_ms[5] += ms_since(t_ph);
+    }
+    // S1: hand every bucket of the rule back (RankingRule::next_bucket serves them one by one): rank, documents, child graph
+    void collect_rule_buckets(QState &q) {
+        Level &L = q.levels.back();
+        const uint64_t W = hix.n_words64;
+        for (size_t ci = 0; ci < L.cost_vals.size(); ci++) {
+            RuleBucket bk;
+            bk.rank = (uint32_t)(L.next_max_cost - L.cost_vals[ci]);
+            bk.max_rank = (uint32_t)L.next_max_cost;
+            bk.count = L.counts[ci];
+            bk.bitmap.assign(W, 0);
+            if (bk.count) {
+                // the activation ran on the dense universe (row j = word j): bucket column ci is a dense bitmap
+                cudaMemcpy(bk.bitmap.data(), L.out + (size_t)ci * L.ld, W * 8, cudaMemcpyDeviceToHost);
+                bk.child = new GraphObj(q.ctx, child_graph(L, ci));
+            }
+            rule_buckets->push_back(std::move(bk));
+        }
+        q.drop_levels();
+        q.done = true;
+    }
     // advance one query's bucket sort until it needs the device again (bucket_sort.rs:193-330)
-    auto emit_bucket = [&](QState &q, Level &L, uint32_t col_lo, uint32_t col_hi, uint64_t count) {
+    void emit_bucket(QState &q, Level &L, uint32_t col_lo, uint32_t col_hi, uint64_t count) {
         if (count == 0) return;
         uint64_t skip = 0;
         uint64_t take = 0;
@@ -2196,69 +2206,13 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         } else
             take = std::min<uint64_t>(count, length - q.n_results);
         if (take) {
-            EmitReq e{};
-            e.d.uw = L.uw;
-            e.d.ub = L.ub;
-            e.d.out = L.out;
-            e.d.rows = L.rows;
-            e.d.ld = L.ld;
-            e.d.col_lo = col_lo;
-            e.d.col_hi = col_hi;
-            e.d.skip = (uint32_t)skip;
-            e.d.take = (uint32_t)take;
-            // dst carries the offset inside the query's result row; the driver turns it into a device pointer
-            e.d.dst = reinterpret_cast<uint32_t *>((uintptr_t)q.n_results);
-            q.emits.push_back(e);
+            q.emits.push_back(emit_desc(q, &L, col_lo, col_hi, skip, take, q.n_results));
             for (uint64_t k = 0; k < take; k++) q.scores.push_back(q.rr_scores);  // bucket_sort.rs:447-455 records them under either strategy
             q.n_results += (uint32_t)take;
         }
         q.cur_offset += count;
-    };
-    auto advance = [&](QState &q) {
-        if (s1 && s1->mode == S1Job::RULE) {
-            // S1: hand every bucket of the rule back (RankingRule::next_bucket serves them one by one): rank, documents, child graph
-            Level &L = q.levels.back();
-            const uint64_t W = hix.n_words64;
-            for (size_t ci = 0; ci < L.cost_vals.size(); ci++) {
-                S1Job::Bucket bk;
-                bk.rank = (uint32_t)(L.next_max_cost - L.cost_vals[ci]);
-                bk.max_rank = (uint32_t)L.next_max_cost;
-                bk.count = L.counts[ci];
-                bk.bitmap.assign(W, 0);
-                if (bk.count) {
-                    // the activation ran on the dense universe (row j = word j): bucket column ci is a dense bitmap
-                    cudaMemcpy(bk.bitmap.data(), L.out + (size_t)ci * L.ld, W * 8, cudaMemcpyDeviceToHost);
-                    GraphObj *child = new GraphObj(hix);
-                    child->ctx.terms = q.ctx.terms;
-                    child->ctx.phrases = q.ctx.phrases;
-                    child->ctx.phrase_ids = q.ctx.phrase_ids;
-                    child->ctx.neg_words = q.ctx.neg_words;
-                    child->ctx.neg_phrases = q.ctx.neg_phrases;
-                    child->ctx.freq_weight = q.ctx.freq_weight;
-                    if (L.kind == RK_EXACT_ATTRIBUTE)
-                        child->graph = L.graph;
-                    else {
-                        std::vector<const SurvPath *> sp;
-                        for (auto &p : L.surv)
-                            if (p.cost_idx == ci) sp.push_back(&p);
-                        std::sort(sp.begin(), sp.end(), [](const SurvPath *x, const SurvPath *y) { return x->edges < y->edges; });
-                        std::vector<std::vector<const ECond *>> good;
-                        for (auto *p : sp) {
-                            std::vector<const ECond *> pc;
-                            for (auto e : p->edges)
-                                if (L.sedges[e].cond >= 0) pc.push_back(&L.conds[L.sedges[e].cond]);
-                            good.push_back(std::move(pc));
-                        }
-                        child->graph = build_from_paths(good);
-                    }
-                    bk.child = child;
-                }
-                s1->buckets.push_back(std::move(bk));
-            }
-            q.drop_levels();
-            q.done = true;
-            return;
-        }
+    }
+    void advance(QState &q) {
         const size_t n_rules = q.rules.size();
         for (;;) {
             if (q.levels.empty()) break;
@@ -2327,17 +2281,7 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                     q.drop_levels();
                     break;
                 }
-                Level C;
-                C.rule_idx = 0;
-                C.kind = q.rules[0];
-                C.graph = q.graph;
-                if (C.kind != RK_EXACT_ATTRIBUTE) {
-                    PROF(1);
-                    prepare_graph_rule(q.ctx, C.kind, C.kind == RK_WORDS, tms, C);
-                }
-                if ((size_t)C.rule_idx + 1 == n_rules) C.want_paths = false;  // nothing descends from the last rule: its buckets are emitted as they are
-                uint32_t cap = (uint32_t)std::min<uint64_t>(cnt, L.rows);
-                request_activation(q, std::move(C), L.uw, L.ub, L.out, L.rows, L.ld, 0, cap);
+                request_activation(q, rule_level(q.ctx, 0, q.rules[0], q.graph, n_rules == 1), ParentRef::bucket(L, 0, cnt));
                 return;
             }
             size_t rule_cur = (size_t)L.rule_idx;
@@ -2392,73 +2336,36 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                 continue;
             }
             // descend: the next rule iterates on this bucket with the query graph of the paths that produced it
-            Level C;
-            C.rule_idx = (int)rule_cur + 1;
-            C.kind = q.rules[rule_cur + 1];
-            if (L.kind == RK_EXACT_ATTRIBUTE)
-                C.graph = L.graph;
-            else {
-                // the paths that took at least one document, in visiting order (= lexicographic in edge ids)
-                PROF(0);
-                if (ci > L.walked_m) {  // cannot happen: buckets 0..walked_m hold every document the query still needed
-                    q.status = B200_ERR_STATE;
-                    q.error = "internal: descent into a bucket whose surviving paths were not computed";
-                    q.drop_levels();
-                    q.done = true;
-                    return;
-                }
-                std::vector<const SurvPath *> sp;
-                for (auto &p : L.surv)
-                    if (p.cost_idx == ci) sp.push_back(&p);
-                std::sort(sp.begin(), sp.end(), [](const SurvPath *x, const SurvPath *y) { return x->edges < y->edges; });
-                std::vector<std::vector<const ECond *>> good;
-                for (auto *p : sp) {
-                    std::vector<const ECond *> pc;
-                    for (auto e : p->edges)
-                        if (L.sedges[e].cond >= 0) pc.push_back(&L.conds[L.sedges[e].cond]);
-                    good.push_back(std::move(pc));
-                }
-                C.graph = build_from_paths(good);
+            if (L.kind != RK_EXACT_ATTRIBUTE && ci > L.walked_m) {  // cannot happen: buckets 0..walked_m hold every document the query still needed
+                q.status = B200_ERR_STATE;
+                q.error = "internal: descent into a bucket whose surviving paths were not computed";
+                q.drop_levels();
+                q.done = true;
+                return;
             }
-            if (C.kind != RK_EXACT_ATTRIBUTE) {
-                PROF(1);
-                prepare_graph_rule(q.ctx, C.kind, false, tms, C);
-            }
-            if ((size_t)C.rule_idx + 1 == n_rules) C.want_paths = false;  // nothing descends from the last rule
-            uint32_t cap = (uint32_t)std::min<uint64_t>(cnt, L.rows);
-            request_activation(q, std::move(C), L.uw, L.ub, L.out, L.rows, L.ld, (uint32_t)ci, cap);
+            request_activation(q, rule_level(q.ctx, (int)rule_cur + 1, q.rules[rule_cur + 1], child_graph(L, ci), rule_cur + 2 == n_rules),
+                               ParentRef::bucket(L, (uint32_t)ci, cnt));
             return;
         }
         q.drop_levels();
         q.done = true;
-    };
+    }
 
     // tree mode: the documents of bucket [col_lo, col_hi) stand at [off, off + cnt) in the query's result order; write the part inside
     // the window [from, from + length) to its final place
-    auto emit_window = [&](QState &q, Level &L, uint32_t col_lo, uint32_t col_hi, uint64_t cnt, uint64_t off, const std::vector<EScore> &sc, ActOut &out) {
+    void emit_window(QState &q, Level &L, uint32_t col_lo, uint32_t col_hi, uint64_t cnt, uint64_t off, const std::vector<EScore> &sc, ActOut &out) {
         const uint64_t win_end = (uint64_t)from + length;
         const uint64_t skip = off < from ? from - off : 0;
         if (skip >= cnt) return;
         const uint64_t start = std::max<uint64_t>(off, from);
         if (start >= win_end) return;
         const uint64_t take = std::min<uint64_t>(cnt - skip, win_end - start);
-        EmitReq e{};
-        e.d.uw = L.uw;
-        e.d.ub = L.ub;
-        e.d.out = L.out;
-        e.d.rows = L.rows;
-        e.d.ld = L.ld;
-        e.d.col_lo = col_lo;
-        e.d.col_hi = col_hi;
-        e.d.skip = (uint32_t)skip;
-        e.d.take = (uint32_t)take;
-        e.d.dst = reinterpret_cast<uint32_t *>((uintptr_t)(start - from));
-        out.emits.push_back(e);
+        out.emits.push_back(emit_desc(q, &L, col_lo, col_hi, skip, take, start - from));
         const size_t at = (size_t)(start - from);  // q.scores was sized when the universe was resolved; windows of different buckets are disjoint
         for (uint64_t k = 0; k < take; k++) q.scores[at + k] = sc;
         out.n_results += (uint32_t)take;
-    };
-    auto release_node = [&](Node *n, ActOut &out) {
+    }
+    static void release_node(Node *n, ActOut &out) {
         Level &L = n->L;
         if (L.a_off != SIZE_MAX) out.freed.emplace_back(L.a_off, L.a_len);
         L.a_off = SIZE_MAX;
@@ -2467,35 +2374,16 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         std::vector<ECond>().swap(L.conds);
         std::vector<SEdge>().swap(L.sedges);
         std::vector<SurvPath>().swap(L.surv);
-    };
+    }
     // tree mode: the activation of node N is complete — place or descend into every bucket of it that reaches the result window
     // (the same decisions as advance(), bucket_sort.rs:193-330, taken for all buckets at once)
-    auto expand = [&](QState &q, Node *N, ActOut &out) {
+    void expand(QState &q, Node *N, ActOut &out) {
         Level &L = N->L;
         // the parent was expanded in an earlier step (self_done); the last of its children to complete gives its buckets back
         if (N->parent && N->parent->live_children.fetch_sub(1) == 1) release_node(N->parent, out);
         const size_t n_rules = q.rules.size();
         const uint64_t win_end = (uint64_t)from + length;
         uint64_t off = N->off0;
-        auto child_graph = [&](Level &C, size_t ci) {
-            if (L.kind == RK_EXACT_ATTRIBUTE) {
-                C.graph = L.graph;
-                return;
-            }
-            PROF(0);
-            std::vector<const SurvPath *> sp;
-            for (auto &p : L.surv)
-                if (p.cost_idx == ci) sp.push_back(&p);
-            std::sort(sp.begin(), sp.end(), [](const SurvPath *x, const SurvPath *y) { return x->edges < y->edges; });
-            std::vector<std::vector<const ECond *>> good;
-            for (auto *p : sp) {
-                std::vector<const ECond *> pc;
-                for (auto e : p->edges)
-                    if (L.sedges[e].cond >= 0) pc.push_back(&L.conds[L.sedges[e].cond]);
-                good.push_back(std::move(pc));
-            }
-            C.graph = build_from_paths(good);
-        };
         if (L.kind == RK_RESOLVE) {
             const uint64_t cnt = L.counts[0];
             q.n_candidates = cnt;
@@ -2504,18 +2392,8 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                 q.scores.resize((size_t)std::min<uint64_t>(length, cnt - from));
                 if (n_rules == 0)
                     emit_window(q, L, 0, 1, cnt, 0, {}, out);
-                else {
-                    Level C;
-                    C.rule_idx = 0;
-                    C.kind = q.rules[0];
-                    C.graph = q.graph;
-                    if (C.kind != RK_EXACT_ATTRIBUTE) {
-                        PROF(1);
-                        prepare_graph_rule(q.ctx, C.kind, C.kind == RK_WORDS, tms, C);
-                    }
-                    if (n_rules == 1) C.want_paths = false;
-                    request_node(q, N, std::move(C), L.uw, L.ub, L.out, L.rows, L.ld, 0, (uint32_t)std::min<uint64_t>(cnt, L.rows), 0, {}, &out);
-                }
+                else
+                    request_node(q, N, rule_level(q.ctx, 0, q.rules[0], q.graph, n_rules == 1), ParentRef::bucket(L, 0, cnt), 0, {}, &out);
             }
         } else {
             const size_t rule_cur = (size_t)L.rule_idx;
@@ -2539,16 +2417,8 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                         out.error = "internal: descent into a bucket whose surviving paths were not computed";
                         return;
                     }
-                    Level C;
-                    C.rule_idx = (int)rule_cur + 1;
-                    C.kind = q.rules[rule_cur + 1];
-                    child_graph(C, ci);
-                    if (C.kind != RK_EXACT_ATTRIBUTE) {
-                        PROF(1);
-                        prepare_graph_rule(q.ctx, C.kind, false, tms, C);
-                    }
-                    if ((size_t)C.rule_idx + 1 == n_rules) C.want_paths = false;  // nothing descends from the last rule
-                    request_node(q, N, std::move(C), L.uw, L.ub, L.out, L.rows, L.ld, (uint32_t)ci, (uint32_t)std::min<uint64_t>(cnt, L.rows), off, sc, &out);
+                    request_node(q, N, rule_level(q.ctx, (int)rule_cur + 1, q.rules[rule_cur + 1], child_graph(L, ci), rule_cur + 2 == n_rules),
+                                 ParentRef::bucket(L, (uint32_t)ci, cnt), off, sc, &out);
                 }
                 sc.pop_back();
                 off += cnt;
@@ -2557,9 +2427,9 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         N->self_done = true;
         if (N->live_children.load() == 0) release_node(N, out);  // no child: nothing will read these buckets after the emissions queued above
         out.expanded = true;
-    };
+    }
     // a query that cannot go on: give everything it holds back
-    auto abandon = [&](QState &q) {
+    static void abandon(QState &q) {
         q.pendings.clear();
         q.emits.clear();
         q.drop_levels();
@@ -2567,102 +2437,97 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         q.nodes.clear();
         q.outstanding = 0;
         q.done = true;
-    };
+    }
 
     // ---- phase 4: step loop.  The batch is split over lanes; every lane has its own stream, device buffers, arena slice, host
     // driver thread and worker sub-pool, so the host phases of one lane overlap both the kernels and the host phases of the others.
     // Drivers are host threads; each alternates between its lanes (software pipeline: while one lane's kernels run, the driver packs
     // and advances its other lane), and the drivers run concurrently.
-    unsigned n_drivers = NQ >= 512 ? 4 : (NQ >= 64 ? 2 : 1), lanes_per_driver = 1;
-    if (const char *env = getenv("B200_DRIVERS")) n_drivers = (unsigned)std::max(1, std::min((int)MAX_DRIVERS, atoi(env)));
-    if (const char *env = getenv("B200_LANES_PER_DRIVER")) lanes_per_driver = (unsigned)std::max(1, atoi(env));
-    if (getenv("B200_SINGLE_LANE")) n_drivers = lanes_per_driver = 1;
-    unsigned n_lanes = std::min<unsigned>(MAX_LANES, n_drivers * lanes_per_driver);
-    if (NQ < n_lanes) n_lanes = n_drivers = lanes_per_driver = 1;
-    lanes_per_driver = n_lanes / n_drivers;
-    {
-        unsigned hw = std::thread::hardware_concurrency();
-        const char *env = getenv("B200_HOST_THREADS");
-        unsigned nt = env ? (unsigned)atoi(env) : std::max(4u, std::min(32u, hw / 2));
-        unsigned per_driver = std::max(1u, nt / n_drivers);
-        for (unsigned dr = 0; dr < n_drivers; dr++) {
-            if (!driver_pools[dr] || driver_pools[dr]->threads.size() + 1 != per_driver) driver_pools[dr].reset(new WorkerPool(per_driver - 1));
-            for (unsigned k = 0; k < lanes_per_driver; k++) lanes[dr * lanes_per_driver + k].pool = driver_pools[dr].get();
-        }
-    }
-    for (unsigned l = 0; l < n_lanes; l++) {
-        Lane &ln = lanes[l];
-        if (!ln.stream) {
-            CU(cudaStreamCreateWithFlags(&ln.stream, cudaStreamNonBlocking), "lane stream");
-            CU(cudaEventCreate(&ln.e0), "lane event");
-            CU(cudaEventCreate(&ln.e1), "lane event");
-            CU(cudaEventCreateWithFlags(&ln.ev_fork, cudaEventDisableTiming), "lane event");
-            for (uint32_t c = 1; c <= EVAL_CLASSES; c++) {
-                CU(cudaStreamCreateWithFlags(&ln.cls_stream[c], cudaStreamNonBlocking), "class stream");
-                CU(cudaEventCreateWithFlags(&ln.ev_join[c], cudaEventDisableTiming), "lane event");
+    int setup_lanes() {
+        CU(eng.d_docids_out.reserve((size_t)NQ * std::max(1u, length)), "alloc results");
+        n_drivers = NQ >= 512 ? 4 : (NQ >= 64 ? 2 : 1);
+        if (const char *env = getenv("B200_DRIVERS")) n_drivers = (unsigned)std::max(1, std::min((int)Engine::MAX_DRIVERS, atoi(env)));
+        if (const char *env = getenv("B200_LANES_PER_DRIVER")) lanes_per_driver = (unsigned)std::max(1, atoi(env));
+        if (getenv("B200_SINGLE_LANE")) n_drivers = lanes_per_driver = 1;
+        n_lanes = std::min<unsigned>(Engine::MAX_LANES, n_drivers * lanes_per_driver);
+        if (NQ < n_lanes) n_lanes = n_drivers = lanes_per_driver = 1;
+        lanes_per_driver = n_lanes / n_drivers;
+        {
+            unsigned per_driver = std::max(1u, host_threads() / n_drivers);
+            for (unsigned dr = 0; dr < n_drivers; dr++) {
+                auto &dp = eng.driver_pools[dr];
+                if (!dp || dp->threads.size() + 1 != per_driver) dp.reset(new WorkerPool(per_driver - 1));
+                for (unsigned k = 0; k < lanes_per_driver; k++) lanes[dr * lanes_per_driver + k].pool = dp.get();
             }
         }
-        ln.scratch = scratch + (((scratch_bytes / n_lanes) * l) & ~(size_t)255);
-        ln.scratch_bytes = (scratch_bytes / n_lanes) & ~(size_t)255;
-        ln.arena = arena + (((arena_bytes / n_lanes) * l) & ~(size_t)255);
-        ln.arena_bytes = (arena_bytes / n_lanes) & ~(size_t)255;
-        ln.alloc.reset(ln.arena_bytes);
-        ln.timing = !(getenv("B200_KERNEL_TIMERS") && atoi(getenv("B200_KERNEL_TIMERS")) == 0);
-        ln.lst = b200_stats{};
-        ln.rc = 0;
-        ln.error.clear();
-        ln.members.clear();
-        ln.inflight = false;
+        for (unsigned l = 0; l < n_lanes; l++) {
+            Lane &ln = lanes[l];
+            if (!ln.stream) {
+                CU(cudaStreamCreateWithFlags(&ln.stream, cudaStreamNonBlocking), "lane stream");
+                CU(cudaEventCreate(&ln.e0), "lane event");
+                CU(cudaEventCreate(&ln.e1), "lane event");
+                CU(cudaEventCreateWithFlags(&ln.ev_fork, cudaEventDisableTiming), "lane event");
+                for (uint32_t c = 1; c <= EVAL_CLASSES; c++) {
+                    CU(cudaStreamCreateWithFlags(&ln.cls_stream[c], cudaStreamNonBlocking), "class stream");
+                    CU(cudaEventCreateWithFlags(&ln.ev_join[c], cudaEventDisableTiming), "lane event");
+                }
+            }
+            ln.scratch = eng.scratch + (((eng.scratch_bytes / n_lanes) * l) & ~(size_t)255);
+            ln.scratch_bytes = (eng.scratch_bytes / n_lanes) & ~(size_t)255;
+            ln.arena = eng.arena + (((eng.arena_bytes / n_lanes) * l) & ~(size_t)255);
+            ln.arena_bytes = (eng.arena_bytes / n_lanes) & ~(size_t)255;
+            ln.alloc.reset(ln.arena_bytes);
+            ln.timing = !(getenv("B200_KERNEL_TIMERS") && atoi(getenv("B200_KERNEL_TIMERS")) == 0);
+            ln.lst = b200_stats{};
+            ln.rc = 0;
+            ln.error.clear();
+            ln.members.clear();
+            ln.inflight = false;
+        }
+        for (unsigned l = 0; l < n_lanes; l++)
+            for (uint32_t i = lane_lo(l); i < lane_lo(l + 1); i++) lanes[l].members.push_back(i);
+        // row lookup tables (scatter_kernel): NQ slots of n_words64 entries, zeroed once per batch.  A lane owns the slots of its query
+        // range and lends each to at most one activation per step; entries carry the tag of the use that wrote them (12 bits, so a slot
+        // serves 4094 steps), which makes the leftovers of earlier uses read as misses.  Activations without a slot search their rows.
+        use_rowtab = hix.n_words64 <= (1u << 20) && !getenv("B200_NO_ROWTAB");
+        if (use_rowtab) {
+            CU(eng.d_rowtab.reserve((size_t)NQ * hix.n_words64), "row lookup tables");
+            CU(cudaMemsetAsync(eng.d_rowtab.p, 0, (size_t)NQ * hix.n_words64 * 4, eng.stream), "zero row lookup tables");
+        }
+        slot_tag.assign(NQ, 0);
+        lane_acts.resize(n_lanes);
+        return B200_OK;
     }
-    auto lane_fail = [&](Lane &ln, int code, const char *msg) {
+    int lane_fail(Lane &ln, int code, const char *msg) {
         ln.error = msg;
         return fail(code, msg);
-    };
-    // contiguous query ranges per lane, so that the first half of the drivers can start while the second half's terms are derived
-    auto lane_lo = [&](unsigned l) { return (uint32_t)((uint64_t)NQ * l / n_lanes); };
-    for (unsigned l = 0; l < n_lanes; l++)
-        for (uint32_t i = lane_lo(l); i < lane_lo(l + 1); i++) lanes[l].members.push_back(i);
-    // row lookup tables (scatter_kernel): NQ slots of n_words64 entries, zeroed once per batch.  A lane owns the slots of its query
-    // range and lends each to at most one activation per step; entries carry the tag of the use that wrote them (12 bits, so a slot
-    // serves 4094 steps), which makes the leftovers of earlier uses read as misses.  Activations without a slot search their rows.
-    const bool use_rowtab = hix.n_words64 <= (1u << 20) && !getenv("B200_NO_ROWTAB");
-    if (use_rowtab) {
-        CU(d_rowtab.reserve((size_t)NQ * hix.n_words64), "row lookup tables");
-        CU(cudaMemsetAsync(d_rowtab.p, 0, (size_t)NQ * hix.n_words64 * 4, stream), "zero row lookup tables");
     }
-    std::vector<uint32_t> slot_tag(NQ, 0);
-    const uint32_t rowtab_min_rows = getenv("B200_ROWTAB_MIN") ? (uint32_t)atoi(getenv("B200_ROWTAB_MIN")) : 64;
-    std::vector<std::vector<std::unique_ptr<Pending>>> lane_acts(n_lanes);
-    const size_t PATH_CAP = (size_t)1 << 20;
-    struct WorkHist {
-        std::mutex mu;
-        uint64_t lists[4][33][2] = {};  // [universe class][log2 card | 32 = dense] -> {lists, stored bytes}
-        uint64_t eval[10][4][4] = {};   // [rule kind][universe class] -> {activations, rows(ld), rows x program ops, rows x columns}
-        uint64_t probes[4] = {};
-    };
-    std::unique_ptr<WorkHist> work_hist_holder(getenv("B200_WORK_HIST") ? new WorkHist() : nullptr);
-    WorkHist *work_hist = work_hist_holder.get();
-    const uint32_t eval_rpt_big = getenv("B200_EVAL_RPT") ? (uint32_t)std::max(1, std::min(8, atoi(getenv("B200_EVAL_RPT")))) : 4;
 
     // pack the pending work of a lane and enqueue it (no synchronisation). returns <0 on error, 0 idle, 1 launched
-    auto launch = [&](Lane &ln) -> int {
+    int launch(Lane &ln) {
         auto t_pack = clk::now();
+        Step s;
+        int rc = schedule(ln, s);
+        if (rc <= 0) return rc;
+        if ((rc = pack(ln, s)) < 0) return rc;
+        if ((rc = enqueue(ln, s)) < 0) return rc;
+        ln.lst.host_ms[3] += ms_since(t_pack);
+        return 1;
+    }
+    // pass 1 (serial, light): which pending activations join the lane's step; their sizes, offsets and device memory.  Returns <0 on
+    // error, 0 when the lane has nothing to do, 1 otherwise.
+    int schedule(Lane &ln, Step &s) {
         ln.act_q.clear();
         const unsigned li = (unsigned)(&ln - lanes);
         std::vector<std::unique_ptr<Pending>> &acts = lane_acts[li];
         acts.clear();
-        struct Cand {
-            uint32_t qi;
-            Pending *pd;
-        };
-        std::vector<uint32_t> emit_q;
-        std::vector<Cand> cand_q;
+        std::vector<Cand> &cand_q = s.cand_q;
         for (auto i : ln.members) {
             QState &q = *qs[i];
             for (auto &f : q.freed) ln.alloc.give(f.first, f.second);  // levels left since the lane's previous step
             q.freed.clear();
             for (auto &pd : q.pendings) cand_q.push_back(Cand{i, pd.get()});
-            if (!q.emits.empty()) emit_q.push_back(i);
+            if (!q.emits.empty()) s.emit_q.push_back(i);
         }
         if (r->candidates)
             for (auto i : ln.members) {  // SearchResult::candidates, copied before any block freed above can be written again
@@ -2676,138 +2541,123 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         // longest first: the parallel-for over these queries ends when its slowest query does, and host time per query grows
         // with the size of its query graph
         std::stable_sort(cand_q.begin(), cand_q.end(), [&](const Cand &x, const Cand &y) { return x.pd->L->graph.nodes.size() > y.pd->L->graph.nodes.size(); });
-        if (cand_q.empty() && emit_q.empty()) return 0;
-        // pass 1 (serial, light): sizes, offsets, device memory
-        struct Plan {
-            uint32_t jobs, sets, words, colprog, states, edges, costs, tiles, probes, res_off, ctiles, n_seg, prog;
-            uint32_t ld, cls, tab_size, rpt, rt_slot, rt_tag;
-            uint8_t *pb;
-            size_t coff, toff, soff_from_end;
-            bool identity;
-        };
-        std::vector<Plan> plan;
-        plan.reserve(cand_q.size());
-        uint32_t n_jobs = 0, n_sets = 0, n_words = 0, n_colprog = 0, n_states = 0, n_edges = 0, n_costs_tot = 0, n_tiles = 0, n_probes = 0, res_words = 0, n_prog = 0;
-        uint32_t n_ctiles = 0, n_tiles_cls[EVAL_CLASSES + 1] = {};
-        bool want_paths_cls[EVAL_CLASSES + 1] = {};
-        bool multi_segment = false;
-        size_t z_used = 0, s_used = 0;
-        uint64_t compact_bytes = 0, eval_bytes = 0, fill_bytes = 0;
+        if (cand_q.empty() && s.emit_q.empty()) return 0;
+        s.plan.reserve(cand_q.size());
         // An activation joins the step when its per-step scratch (condition matrix, DP table, path table) and its persistent block
         // (universe rows + bucket columns) fit; otherwise it waits for a later step of the lane (scratch is reused every step, the
         // arena is refilled as queries leave levels).  New queries (first activation) are only admitted while the arena is less
         // than ~60 % full, so that the queries already descending can finish.  When nothing at all fits and the lane is idle, the
         // waiting query with the largest demand fails alone with B200_ERR_CAPACITY and the others go on.
         bool admit_all = false;
-        std::vector<size_t> sched;  // indices in cand_q of the activations that join this step
         uint32_t next_slot = lane_lo(li);
         const uint32_t slot_end = lane_lo(li + 1);
-    plan_again:
-        for (size_t ci = 0; ci < cand_q.size(); ci++) {
-            Pending &pd = *cand_q[ci].pd;
-            StepOut &o = pd.o;
-            Plan pl{};
-            pl.jobs = n_jobs;
-            pl.sets = n_sets;
-            pl.words = n_words;
-            pl.colprog = n_colprog;
-            pl.states = n_states;
-            pl.edges = n_edges;
-            pl.costs = n_costs_tot;
-            pl.prog = n_prog;
-            pl.probes = n_probes;
-            pl.res_off = res_words;
-            uint32_t ld = std::max(1u, pd.p_cap);
-            pl.ld = ld;
-            pl.identity = !pd.p_uw && !pd.p_out;  // first activation of a query: the universe is the dense documents bitmap itself
-            uint32_t n_cols = std::max(1u, o.n_cols);
-            uint32_t tab_size = o.want_paths ? 4096u << pd.tab_shift : 1;
-            pl.tab_size = tab_size;
-            pl.cls = eval_class(n_cols + o.n_pairs + EVAL_EXTRA_SLOTS);
-            pl.rpt = 1;  // rows per thread: > 1 only pays for grids far larger than the GPU (it lengthens the tail of small grids); measured
-                         // at 10 M documents: 4 rows per thread on the >= 65536-row activations of the smallest class saves 15 % of the pass
-            if (eval_rpt_big > 1 && pl.cls == 0 && ld >= 65536) pl.rpt = eval_rpt_big;
-            const uint32_t my_tiles = (ld + 128 * pl.rpt - 1) / (128 * pl.rpt);
-            size_t persist = pl.identity ? (size_t)ld * 8 * (o.n_costs + 1) : (size_t)ld * 4 + 256 + (size_t)ld * 8 + 256 + (size_t)ld * 8 * (o.n_costs + 1);
-            size_t cbytes = (size_t)ld * 8 * n_cols, sbytes = pl.cls < EVAL_CLASSES ? 0 : (size_t)ld * 8 * o.n_pairs, tbytes = (size_t)tab_size * 8;
-            // zeroed zone (condition matrix + path table) grows from the front of the lane's scratch, the DP table from the back
-            pl.coff = (z_used + 255) & ~(size_t)255;
-            pl.toff = (pl.coff + cbytes + 255) & ~(size_t)255;
-            size_t s_need = (sbytes + 255) & ~(size_t)255;
-            pd.demand = persist + cbytes + tbytes + s_need;
-            if (pl.toff + tbytes + s_need + s_used > ln.scratch_bytes) continue;                  // next step
-            if (pl.identity && !admit_all && ln.alloc.used * 5 > ln.alloc.total * 3) continue;  // admission
-            size_t aoff = ln.alloc.take(persist);
-            if (aoff == SIZE_MAX) continue;
-            pl.pb = ln.arena + aoff;
-            pd.L->a_off = aoff;
-            pd.L->a_len = persist;
-            pl.rt_slot = UINT32_MAX;
-            if (use_rowtab && !pl.identity && ld >= rowtab_min_rows) {
-                while (next_slot < slot_end && slot_tag[next_slot] >= 4094) next_slot++;
-                if (next_slot < slot_end) {
-                    pl.rt_slot = next_slot;
-                    pl.rt_tag = ++slot_tag[next_slot];
-                    next_slot++;
+        for (;;) {
+            for (size_t ci = 0; ci < cand_q.size(); ci++) {
+                Pending &pd = *cand_q[ci].pd;
+                StepOut &o = pd.o;
+                Plan pl{};
+                pl.jobs = s.n_jobs;
+                pl.sets = s.n_sets;
+                pl.words = s.n_words;
+                pl.colprog = s.n_colprog;
+                pl.states = s.n_states;
+                pl.edges = s.n_edges;
+                pl.costs = s.n_costs_tot;
+                pl.prog = s.n_prog;
+                pl.probes = s.n_probes;
+                pl.res_off = s.res_words;
+                uint32_t ld = std::max(1u, pd.parent.cap);
+                pl.ld = ld;
+                pl.identity = !pd.parent.uw && !pd.parent.out;  // first activation of a query: the universe is the dense documents bitmap itself
+                uint32_t n_cols = std::max(1u, o.n_cols);
+                uint32_t tab_size = o.want_paths ? 4096u << pd.tab_shift : 1;
+                pl.tab_size = tab_size;
+                pl.cls = eval_class(n_cols + o.n_pairs + EVAL_EXTRA_SLOTS);
+                pl.rpt = 1;  // rows per thread: > 1 only pays for grids far larger than the GPU (it lengthens the tail of small grids); measured
+                             // at 10 M documents: 4 rows per thread on the >= 65536-row activations of the smallest class saves 15 % of the pass
+                if (eval_rpt_big > 1 && pl.cls == 0 && ld >= 65536) pl.rpt = eval_rpt_big;
+                const uint32_t my_tiles = (ld + 128 * pl.rpt - 1) / (128 * pl.rpt);
+                size_t persist = pl.identity ? (size_t)ld * 8 * (o.n_costs + 1) : (size_t)ld * 4 + 256 + (size_t)ld * 8 + 256 + (size_t)ld * 8 * (o.n_costs + 1);
+                size_t cbytes = (size_t)ld * 8 * n_cols, sbytes = pl.cls < EVAL_CLASSES ? 0 : (size_t)ld * 8 * o.n_pairs, tbytes = (size_t)tab_size * 8;
+                // zeroed zone (condition matrix + path table) grows from the front of the lane's scratch, the DP table from the back
+                pl.coff = (s.z_used + 255) & ~(size_t)255;
+                pl.toff = (pl.coff + cbytes + 255) & ~(size_t)255;
+                size_t s_need = (sbytes + 255) & ~(size_t)255;
+                pd.demand = persist + cbytes + tbytes + s_need;
+                if (pl.toff + tbytes + s_need + s.s_used > ln.scratch_bytes) continue;               // next step
+                if (pl.identity && !admit_all && ln.alloc.used * 5 > ln.alloc.total * 3) continue;  // admission
+                size_t aoff = ln.alloc.take(persist);
+                if (aoff == SIZE_MAX) continue;
+                pl.pb = ln.arena + aoff;
+                pd.L->a_off = aoff;
+                pd.L->a_len = persist;
+                pl.rt_slot = UINT32_MAX;
+                if (use_rowtab && !pl.identity && ld >= rowtab_min_rows) {
+                    while (next_slot < slot_end && slot_tag[next_slot] >= 4094) next_slot++;
+                    if (next_slot < slot_end) {
+                        pl.rt_slot = next_slot;
+                        pl.rt_tag = ++slot_tag[next_slot];
+                        next_slot++;
+                    }
                 }
-            }
-            n_jobs += (uint32_t)o.jobs.size();
-            n_sets += (uint32_t)o.pairsets.size();
-            n_words += (uint32_t)o.words.size();
-            n_colprog += (uint32_t)o.colprog.size();
-            n_states += (uint32_t)o.dp_states.size();
-            n_edges += (uint32_t)o.dp_edges.size();
-            n_costs_tot += (uint32_t)o.cost_vals.size();
-            n_prog += (uint32_t)o.prog.size();
-            want_paths_cls[pl.cls] = want_paths_cls[pl.cls] || o.want_paths;
-            pl.tiles = n_tiles_cls[pl.cls];  // within its class; the class bases are added below
-            n_tiles_cls[pl.cls] += my_tiles;
-            n_tiles += my_tiles;
-            for (auto &ps : o.pairsets) n_probes += ps.n_left * ps.n_right;
-            res_words += 4 + o.n_costs;  // rows | n_costs + 1 bucket counts | path-table saturation flag | last walked bucket
-            pl.n_seg = pl.identity ? 1u : std::max(1u, (pd.p_rows + COMPACT_SEG - 1) / COMPACT_SEG);
-            pl.ctiles = n_ctiles;
-            n_ctiles += pl.n_seg;
-            multi_segment = multi_segment || pl.n_seg > 1;
-            z_used = pl.toff + tbytes;
-            s_used += s_need;
-            pl.soff_from_end = s_used;
-            ln.act_q.push_back(cand_q[ci].qi);
-            sched.push_back(ci);
-            ln.lst.posting_bytes += o.posting_bytes;
-            // algorithmic bytes of the evaluation: condition columns in, universe word in, bucket columns out (the DP table is on-chip)
-            uint64_t mb = (uint64_t)ld * 8 * (n_cols + o.n_costs + 2);
-            ln.lst.matrix_bytes += mb;
-            eval_bytes += mb;
-            if (!pl.identity) compact_bytes += (uint64_t)pd.p_rows * 8 + (uint64_t)ld * 12;
-            fill_bytes += o.posting_bytes;
-            if (work_hist) {  // B200_WORK_HIST=1: where the step's work comes from (developer statistics, see tools/)
-                const int kind = pd.L->kind;
-                const int ub = ld >= 65536 ? 3 : (ld >= 4096 ? 2 : (ld >= 128 ? 1 : 0));
-                std::lock_guard<std::mutex> g(work_hist->mu);
-                for (auto &jb : o.jobs) {
-                    if (jb.chunk) continue;
-                    const ListRef &lr = hix.lists[jb.list];
-                    int cb = 0;
-                    while ((1u << cb) < lr.card && cb < 31) cb++;
-                    auto &cell = work_hist->lists[ub][lr.dense ? 32 : cb];
-                    cell[0]++;
-                    cell[1] += lr.dense ? (uint64_t)hix.n_words64 * 8 : (uint64_t)lr.card * 4;
+                s.n_jobs += (uint32_t)o.jobs.size();
+                s.n_sets += (uint32_t)o.pairsets.size();
+                s.n_words += (uint32_t)o.words.size();
+                s.n_colprog += (uint32_t)o.colprog.size();
+                s.n_states += (uint32_t)o.dp_states.size();
+                s.n_edges += (uint32_t)o.dp_edges.size();
+                s.n_costs_tot += (uint32_t)o.cost_vals.size();
+                s.n_prog += (uint32_t)o.prog.size();
+                s.want_paths_cls[pl.cls] = s.want_paths_cls[pl.cls] || o.want_paths;
+                pl.tiles = s.n_tiles_cls[pl.cls];  // within its class; the class bases are added below
+                s.n_tiles_cls[pl.cls] += my_tiles;
+                s.n_tiles += my_tiles;
+                for (auto &ps : o.pairsets) s.n_probes += ps.n_left * ps.n_right;
+                s.res_words += 4 + o.n_costs;  // rows | n_costs + 1 bucket counts | path-table saturation flag | last walked bucket
+                pl.n_seg = pl.identity ? 1u : std::max(1u, (pd.parent.rows + COMPACT_SEG - 1) / COMPACT_SEG);
+                pl.ctiles = s.n_ctiles;
+                s.n_ctiles += pl.n_seg;
+                s.multi_segment = s.multi_segment || pl.n_seg > 1;
+                s.z_used = pl.toff + tbytes;
+                s.s_used += s_need;
+                pl.soff_from_end = s.s_used;
+                ln.act_q.push_back(cand_q[ci].qi);
+                s.sched.push_back(ci);
+                ln.lst.posting_bytes += o.posting_bytes;
+                // algorithmic bytes of the evaluation: condition columns in, universe word in, bucket columns out (the DP table is on-chip)
+                uint64_t mb = (uint64_t)ld * 8 * (n_cols + o.n_costs + 2);
+                ln.lst.matrix_bytes += mb;
+                s.eval_bytes += mb;
+                if (!pl.identity) s.compact_bytes += (uint64_t)pd.parent.rows * 8 + (uint64_t)ld * 12;
+                s.fill_bytes += o.posting_bytes;
+                if (work_hist) {  // B200_WORK_HIST=1: where the step's work comes from (developer statistics, see tools/)
+                    const int kind = pd.L->kind;
+                    const int ub = ld >= 65536 ? 3 : (ld >= 4096 ? 2 : (ld >= 128 ? 1 : 0));
+                    std::lock_guard<std::mutex> g(work_hist->mu);
+                    for (auto &jb : o.jobs) {
+                        if (jb.chunk) continue;
+                        const ListRef &lr = hix.lists[jb.list];
+                        int cb = 0;
+                        while ((1u << cb) < lr.card && cb < 31) cb++;
+                        auto &cell = work_hist->lists[ub][lr.dense ? 32 : cb];
+                        cell[0]++;
+                        cell[1] += lr.dense ? (uint64_t)hix.n_words64 * 8 : (uint64_t)lr.card * 4;
+                    }
+                    auto &ev = work_hist->eval[kind][ub];
+                    ev[0]++;
+                    ev[1] += ld;
+                    ev[2] += (uint64_t)ld * o.prog.size();
+                    ev[3] += (uint64_t)ld * n_cols;
+                    for (auto &ps : o.pairsets) work_hist->probes[ub] += (uint64_t)ps.n_left * ps.n_right;
                 }
-                auto &ev = work_hist->eval[kind][ub];
-                ev[0]++;
-                ev[1] += ld;
-                ev[2] += (uint64_t)ld * o.prog.size();
-                ev[3] += (uint64_t)ld * n_cols;
-                for (auto &ps : o.pairsets) work_hist->probes[ub] += (uint64_t)ps.n_left * ps.n_right;
+                s.plan.push_back(pl);
             }
-            plan.push_back(pl);
-        }
-        if (ln.act_q.empty() && emit_q.empty()) {
-            // the lane is idle (launch is only called between its steps) and nothing fits
+            if (!ln.act_q.empty() || !s.emit_q.empty()) break;
+            // the lane is idle (launch is only called between its steps) and nothing fits; nothing was scheduled, so the pass
+            // starts over from the same state
             if (!admit_all) {
                 admit_all = true;
-                goto plan_again;
+                continue;
             }
             size_t worst = 0;
             for (size_t k = 1; k < cand_q.size(); k++)
@@ -2823,11 +2673,10 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             ln.lst.deferred++;
             if (cand_q.empty()) return 0;
             admit_all = false;
-            goto plan_again;
         }
         ln.lst.deferred += cand_q.size() - ln.act_q.size();
         // the scheduled activations leave their queries' pending lists for the lane's step
-        for (auto ci : sched) {
+        for (auto ci : s.sched) {
             QState &q = *qs[cand_q[ci].qi];
             for (auto &up : q.pendings)
                 if (up.get() == cand_q[ci].pd) {
@@ -2835,18 +2684,20 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                     break;
                 }
         }
-        for (auto ci : sched) {
+        for (auto ci : s.sched) {
             auto &pv = qs[cand_q[ci].qi]->pendings;
             pv.erase(std::remove(pv.begin(), pv.end(), nullptr), pv.end());
         }
-        uint32_t tile_base[EVAL_CLASSES + 2] = {};
-        for (uint32_t c = 0; c <= EVAL_CLASSES; c++) tile_base[c + 1] = tile_base[c] + n_tiles_cls[c];
-        for (auto &pl : plan) pl.tiles += tile_base[pl.cls];
+        for (uint32_t c = 0; c <= EVAL_CLASSES; c++) s.tile_base[c + 1] = s.tile_base[c] + s.n_tiles_cls[c];
+        for (auto &pl : s.plan) pl.tiles += s.tile_base[pl.cls];
+        return 1;
+    }
+    // pass 2 (parallel): the step blob, written straight into the lane's pinned buffer
+    int pack(Lane &ln, Step &s) {
         ln.lst.device_steps++;
-        const std::vector<uint32_t> &act_q = ln.act_q;
-        const size_t NA = act_q.size();
-        uint32_t n_emits = 0;
-        for (auto qi : emit_q) n_emits += (uint32_t)qs[qi]->emits.size();
+        const std::vector<std::unique_ptr<Pending>> &acts = lane_acts[(unsigned)(&ln - lanes)];
+        const size_t NA = ln.act_q.size();
+        for (auto qi : s.emit_q) s.n_emits += (uint32_t)qs[qi]->emits.size();
         // section offsets inside the step blob
         size_t off = 0;
         auto section = [&](size_t bytes) {
@@ -2854,34 +2705,40 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             off = o0 + bytes;
             return o0;
         };
-        size_t o_acts = section(NA * sizeof(ActDesc)), o_sets = section((size_t)n_sets * sizeof(PairSet)), o_words = section((size_t)n_words * 4),
-               o_colprog = section((size_t)n_colprog * sizeof(ColOp)), o_states = section((size_t)n_states * sizeof(DpState)),
-               o_edges = section((size_t)n_edges * sizeof(DpEdge)), o_costs = section((size_t)n_costs_tot * 2), o_prog = section((size_t)n_prog * 4),
-               o_tiles = section((size_t)n_tiles * sizeof(TileDesc)), o_ctiles = section((size_t)n_ctiles * sizeof(CompactTile)),
-               o_emits = section((size_t)n_emits * sizeof(EmitDesc)),
-               o_jobs = section((size_t)n_jobs * sizeof(Job)), o_nstatic = section(16);
-        size_t nbytes = off + 16;
-        if (nbytes > ln.h_step_cap) {
+        s.o_acts = section(NA * sizeof(ActDesc));
+        s.o_sets = section((size_t)s.n_sets * sizeof(PairSet));
+        s.o_words = section((size_t)s.n_words * 4);
+        s.o_colprog = section((size_t)s.n_colprog * sizeof(ColOp));
+        s.o_states = section((size_t)s.n_states * sizeof(DpState));
+        s.o_edges = section((size_t)s.n_edges * sizeof(DpEdge));
+        s.o_costs = section((size_t)s.n_costs_tot * 2);
+        s.o_prog = section((size_t)s.n_prog * 4);
+        s.o_tiles = section((size_t)s.n_tiles * sizeof(TileDesc));
+        s.o_ctiles = section((size_t)s.n_ctiles * sizeof(CompactTile));
+        s.o_emits = section((size_t)s.n_emits * sizeof(EmitDesc));
+        s.o_jobs = section((size_t)s.n_jobs * sizeof(Job));
+        s.o_nstatic = section(16);
+        s.nbytes = off + 16;
+        if (s.nbytes > ln.h_step_cap) {
             if (ln.h_step) cudaFreeHost(ln.h_step);
-            ln.h_step_cap = nbytes * 2;
+            ln.h_step_cap = s.nbytes * 2;
             CU(cudaMallocHost((void **)&ln.h_step, ln.h_step_cap), "pinned step buffer");
         }
         uint8_t *hb = ln.h_step;
-        // pass 2 (parallel): write every activation's slice of the blob straight into pinned memory
         ln.pool->run(NA, [&](size_t a) {
             Pending &pd = *acts[a];
             Level &L = *pd.L;
             StepOut &o = pd.o;
-            const Plan &pl = plan[a];
+            const Plan &pl = s.plan[a];
             ActDesc d;
             memset(&d, 0, sizeof d);
-            d.p_uw = pd.p_uw;
-            d.p_ub = pd.p_ub;
-            d.p_out = pd.p_out;
-            d.p_rows = pd.p_rows;
-            d.p_ld = pd.p_ld;
-            d.p_col_lo = pd.p_col;
-            d.p_col_hi = pd.p_col + 1;
+            d.p_uw = pd.parent.uw;
+            d.p_ub = pd.parent.ub;
+            d.p_out = pd.parent.out;
+            d.p_rows = pd.parent.rows;
+            d.p_ld = pd.parent.ld;
+            d.p_col_lo = pd.parent.col;
+            d.p_col_hi = pd.parent.col + 1;
             uint32_t ld = pl.ld;
             d.ld = ld;
             d.n_cols = std::max(1u, o.n_cols);
@@ -2895,7 +2752,7 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             d.C = reinterpret_cast<unsigned long long *>(ln.scratch + pl.coff);
             if (pl.identity) {
                 d.uw = nullptr;
-                d.ub = const_cast<unsigned long long *>(pd.p_ub);
+                d.ub = const_cast<unsigned long long *>(pd.parent.ub);
                 d.out = reinterpret_cast<unsigned long long *>(pl.pb);
             } else {
                 d.uw = reinterpret_cast<uint32_t *>(pl.pb);
@@ -2906,7 +2763,7 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             d.row_tag = 0;
             if (pl.rt_slot != UINT32_MAX) {
                 d.row_tag = pl.rt_tag;
-                d.row_tab = d_rowtab.p + (size_t)pl.rt_slot * hix.n_words64;
+                d.row_tab = eng.d_rowtab.p + (size_t)pl.rt_slot * hix.n_words64;
             }
             L.uw = d.uw;
             L.ub = d.ub;
@@ -2923,21 +2780,21 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             d.need = pd.need;
             d.root_rmin = o.dp_states.empty() ? 0 : o.dp_states[0].rmin;
             d.root_rcount = o.dp_states.empty() ? 0 : o.dp_states[0].rcount;
-            if (!o.prog.empty()) memcpy(hb + o_prog + (size_t)pl.prog * 4, o.prog.data(), o.prog.size() * 4);
+            if (!o.prog.empty()) memcpy(hb + s.o_prog + (size_t)pl.prog * 4, o.prog.data(), o.prog.size() * 4);
             d.res_off = pl.res_off;
             L.res_off = pl.res_off;
-            memcpy(hb + o_acts + a * sizeof(ActDesc), &d, sizeof d);
-            if (!o.colprog.empty()) memcpy(hb + o_colprog + (size_t)pl.colprog * sizeof(ColOp), o.colprog.data(), o.colprog.size() * sizeof(ColOp));
-            if (!o.dp_states.empty()) memcpy(hb + o_states + (size_t)pl.states * sizeof(DpState), o.dp_states.data(), o.dp_states.size() * sizeof(DpState));
-            if (!o.dp_edges.empty()) memcpy(hb + o_edges + (size_t)pl.edges * sizeof(DpEdge), o.dp_edges.data(), o.dp_edges.size() * sizeof(DpEdge));
-            if (!o.cost_vals.empty()) memcpy(hb + o_costs + (size_t)pl.costs * 2, o.cost_vals.data(), o.cost_vals.size() * 2);
-            if (!o.words.empty()) memcpy(hb + o_words + (size_t)pl.words * 4, o.words.data(), o.words.size() * 4);
-            Job *jd = reinterpret_cast<Job *>(hb + o_jobs) + pl.jobs;
+            memcpy(hb + s.o_acts + a * sizeof(ActDesc), &d, sizeof d);
+            if (!o.colprog.empty()) memcpy(hb + s.o_colprog + (size_t)pl.colprog * sizeof(ColOp), o.colprog.data(), o.colprog.size() * sizeof(ColOp));
+            if (!o.dp_states.empty()) memcpy(hb + s.o_states + (size_t)pl.states * sizeof(DpState), o.dp_states.data(), o.dp_states.size() * sizeof(DpState));
+            if (!o.dp_edges.empty()) memcpy(hb + s.o_edges + (size_t)pl.edges * sizeof(DpEdge), o.dp_edges.data(), o.dp_edges.size() * sizeof(DpEdge));
+            if (!o.cost_vals.empty()) memcpy(hb + s.o_costs + (size_t)pl.costs * 2, o.cost_vals.data(), o.cost_vals.size() * 2);
+            if (!o.words.empty()) memcpy(hb + s.o_words + (size_t)pl.words * 4, o.words.data(), o.words.size() * 4);
+            Job *jd = reinterpret_cast<Job *>(hb + s.o_jobs) + pl.jobs;
             for (size_t k = 0; k < o.jobs.size(); k++) {
                 jd[k] = o.jobs[k];
                 jd[k].act = (uint32_t)a;
             }
-            PairSet *sd = reinterpret_cast<PairSet *>(hb + o_sets) + pl.sets;
+            PairSet *sd = reinterpret_cast<PairSet *>(hb + s.o_sets) + pl.sets;
             uint32_t pb = pl.probes;
             for (size_t k = 0; k < o.pairsets.size(); k++) {
                 sd[k] = o.pairsets[k];
@@ -2947,32 +2804,39 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                 sd[k].probe_base = pb;
                 pb += sd[k].n_left * sd[k].n_right;
             }
-            TileDesc *td = reinterpret_cast<TileDesc *>(hb + o_tiles) + pl.tiles;
+            TileDesc *td = reinterpret_cast<TileDesc *>(hb + s.o_tiles) + pl.tiles;
             for (uint32_t r0 = 0, k = 0; r0 < ld; r0 += 128 * pl.rpt, k++) td[k] = TileDesc{(uint32_t)a, r0, pl.rpt, 0};
-            CompactTile *ct = reinterpret_cast<CompactTile *>(hb + o_ctiles) + pl.ctiles;
+            CompactTile *ct = reinterpret_cast<CompactTile *>(hb + s.o_ctiles) + pl.ctiles;
             for (uint32_t sg = 0; sg < pl.n_seg; sg++) ct[sg] = CompactTile{(uint32_t)a, sg, pl.ctiles, pl.n_seg};
         });
         {
-            EmitDesc *ed = reinterpret_cast<EmitDesc *>(hb + o_emits);
+            EmitDesc *ed = reinterpret_cast<EmitDesc *>(hb + s.o_emits);
             size_t k = 0;
-            for (auto qi : emit_q) {
+            for (auto qi : s.emit_q) {
                 QState &q = *qs[qi];
                 for (auto &e : q.emits) {
-                    EmitDesc d = e.d;
-                    d.dst = d_docids_out.p + (size_t)qi * std::max(1u, length) + (uint32_t)(uintptr_t)e.d.dst;
+                    EmitDesc d = e;
+                    d.dst = eng.d_docids_out.p + (size_t)qi * std::max(1u, length) + (uint32_t)(uintptr_t)e.dst;
                     ed[k++] = d;
                 }
                 q.emits.clear();
             }
         }
-        uint32_t n_static = n_jobs;
-        memcpy(hb + o_nstatic, &n_static, 4);
+        uint32_t n_static = s.n_jobs;
+        memcpy(hb + s.o_nstatic, &n_static, 4);
+        return B200_OK;
+    }
+    // the step's copies and kernels on the lane's streams
+    int enqueue(Lane &ln, const Step &s) {
+        const size_t NA = ln.act_q.size();
+        const uint32_t res_words = s.res_words, n_tiles = s.n_tiles, n_ctiles = s.n_ctiles, n_emits = s.n_emits;
+        const size_t nbytes = s.nbytes;
         CU(ln.d_step.reserve(nbytes), "step buffer");
         cudaStream_t st = ln.stream;
         CU(cudaMemcpyAsync(ln.d_step.p, ln.h_step, nbytes, cudaMemcpyHostToDevice, st), "H2D step");
         ln.lst.h2d_bytes += nbytes;
         ln.lst.d2h_bytes += (size_t)res_words * 4 + 8;
-        size_t qcap = std::max<size_t>((size_t)n_jobs + ((size_t)1 << 20), (size_t)4 << 20);
+        size_t qcap = std::max<size_t>((size_t)s.n_jobs + ((size_t)1 << 20), (size_t)4 << 20);
         CU(ln.d_queue.reserve(qcap), "job queue");
         qcap = ln.d_queue.cap;
         CU(ln.d_qcount.reserve(8), "job counter");
@@ -2982,75 +2846,75 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             ln.h_results_cap = (size_t)(res_words + 4) * 2;
             CU(cudaMallocHost((void **)&ln.h_results, ln.h_results_cap * 4), "pinned results");
         }
-        if (n_jobs) CU(cudaMemcpyAsync(ln.d_queue.p, ln.d_step.p + o_jobs, (size_t)n_jobs * sizeof(Job), cudaMemcpyDeviceToDevice, st), "jobs to queue");
-        CU(cudaMemcpyAsync(ln.d_qcount.p, ln.d_step.p + o_nstatic, 4, cudaMemcpyDeviceToDevice, st), "job count");
-        const ActDesc *dacts = reinterpret_cast<const ActDesc *>(ln.d_step.p + o_acts);
+        if (s.n_jobs) CU(cudaMemcpyAsync(ln.d_queue.p, ln.d_step.p + s.o_jobs, (size_t)s.n_jobs * sizeof(Job), cudaMemcpyDeviceToDevice, st), "jobs to queue");
+        CU(cudaMemcpyAsync(ln.d_qcount.p, ln.d_step.p + s.o_nstatic, 4, cudaMemcpyDeviceToDevice, st), "job count");
+        const ActDesc *dacts = reinterpret_cast<const ActDesc *>(ln.d_step.p + s.o_acts);
         // 1. emissions queued before this step's activations
         if (ln.timing) CU(cudaEventRecord(ln.e0, st), "event");
         if (n_emits) {
             size_t m0 = ln.mark();
-            CU(launch_emit(st, reinterpret_cast<const EmitDesc *>(ln.d_step.p + o_emits), n_emits), "emit");
+            CU(launch_emit(st, reinterpret_cast<const EmitDesc *>(ln.d_step.p + s.o_emits), n_emits), "emit");
             ln.time_kernel(ln.lst, B200_K_EMIT, m0, ln.mark(), (uint64_t)n_emits * 64);
         }
         if (NA) {
             CU(cudaMemsetAsync(ln.d_results.p, 0, (size_t)(res_words + 4) * 4, st), "zero results");
-            CU(cudaMemsetAsync(ln.scratch, 0, z_used, st), "zero condition matrix");
+            CU(cudaMemsetAsync(ln.scratch, 0, s.z_used, st), "zero condition matrix");
             CU(ln.d_pathbuf.reserve(PATH_CAP), "path buffer");
             CU(cudaMemsetAsync(ln.d_qcount.p + 1, 0, 16, st), "zero path count and the scatter cursors");
             size_t t0 = ln.mark();
             CU(ln.d_segcount.reserve(n_ctiles + 1), "segment counts");
-            CU(launch_compact(st, reinterpret_cast<const CompactTile *>(ln.d_step.p + o_ctiles), n_ctiles, multi_segment, dacts, ln.d_segcount.p,
+            CU(launch_compact(st, reinterpret_cast<const CompactTile *>(ln.d_step.p + s.o_ctiles), n_ctiles, s.multi_segment, dacts, ln.d_segcount.p,
                               ln.d_results.p),
                "compact");
-            if (multi_segment) ln.lst.kernel_launches++;  // act_count_kernel
+            if (s.multi_segment) ln.lst.kernel_launches++;  // act_count_kernel
             size_t t1 = ln.mark();
-            ln.time_kernel(ln.lst, B200_K_COMPACT, t0, t1, compact_bytes);
-            CU(launch_pair_probe(st, reinterpret_cast<const PairSet *>(ln.d_step.p + o_sets), n_sets, n_probes,
-                                 reinterpret_cast<const uint32_t *>(ln.d_step.p + o_words), dix.pair_keys, hix.pair_keys.size(), hix.pair_list_base,
+            ln.time_kernel(ln.lst, B200_K_COMPACT, t0, t1, s.compact_bytes);
+            CU(launch_pair_probe(st, reinterpret_cast<const PairSet *>(ln.d_step.p + s.o_sets), s.n_sets, s.n_probes,
+                                 reinterpret_cast<const uint32_t *>(ln.d_step.p + s.o_words), dix.pair_keys, hix.pair_keys.size(), hix.pair_list_base,
                                  dix.lists, dacts, ln.d_results.p, ln.d_queue.p, ln.d_qcount.p, (uint32_t)qcap),
                "pair probe");
             size_t t2 = ln.mark();
-            if (n_probes) ln.time_kernel(ln.lst, B200_K_PAIR_PROBE, t1, t2, (uint64_t)n_probes * 8 * 23);
+            if (s.n_probes) ln.time_kernel(ln.lst, B200_K_PAIR_PROBE, t1, t2, (uint64_t)s.n_probes * 8 * 23);
             CU(ln.d_bigq.reserve(qcap), "big-job queue");
-            CU(launch_scatter(st, (uint32_t)sm_count * 5, ln.d_queue.p, ln.d_qcount.p, (uint32_t)qcap, dacts, ln.d_results.p, dix.lists, dix.pool,
+            CU(launch_scatter(st, (uint32_t)eng.sm_count * 5, ln.d_queue.p, ln.d_qcount.p, (uint32_t)qcap, dacts, ln.d_results.p, dix.lists, dix.pool,
                               ln.d_bigq.p),
                "scatter");
             ln.lst.kernel_launches++;
             size_t t3 = ln.mark();
-            ln.time_kernel(ln.lst, B200_K_SCATTER, t2, t3, fill_bytes);
+            ln.time_kernel(ln.lst, B200_K_SCATTER, t2, t3, s.fill_bytes);
             // the classes are independent (different activations): class 0 stays on the lane's stream, the others run beside it on
             // forked streams and are joined before the results are copied back
             CU(ln.d_tile_summary.reserve(2 * (size_t)n_tiles + 2), "tile summaries");
             uint32_t n_forked = 0;
-            for (uint32_t c = 1; c <= EVAL_CLASSES; c++) n_forked += n_tiles_cls[c] ? 1 : 0;
+            for (uint32_t c = 1; c <= EVAL_CLASSES; c++) n_forked += s.n_tiles_cls[c] ? 1 : 0;
             if (n_forked) CU(cudaEventRecord(ln.ev_fork, st), "fork");
             for (uint32_t c = 0; c <= EVAL_CLASSES; c++) {
-                if (!n_tiles_cls[c]) continue;
+                if (!s.n_tiles_cls[c]) continue;
                 cudaStream_t cs = c == 0 ? st : ln.cls_stream[c];
                 if (c) CU(cudaStreamWaitEvent(cs, ln.ev_fork, 0), "fork wait");
-                const TileDesc *tl = reinterpret_cast<const TileDesc *>(ln.d_step.p + o_tiles) + tile_base[c];
-                CU(launch_eval(cs, (int)c, tl, n_tiles_cls[c], dacts, ln.d_results.p, reinterpret_cast<const ColOp *>(ln.d_step.p + o_colprog),
-                               reinterpret_cast<const uint16_t *>(ln.d_step.p + o_costs), reinterpret_cast<const uint32_t *>(ln.d_step.p + o_prog),
-                               ln.d_tile_summary.p + 2 * (size_t)tile_base[c]),
+                const TileDesc *tl = reinterpret_cast<const TileDesc *>(ln.d_step.p + s.o_tiles) + s.tile_base[c];
+                CU(launch_eval(cs, (int)c, tl, s.n_tiles_cls[c], dacts, ln.d_results.p, reinterpret_cast<const ColOp *>(ln.d_step.p + s.o_colprog),
+                               reinterpret_cast<const uint16_t *>(ln.d_step.p + s.o_costs), reinterpret_cast<const uint32_t *>(ln.d_step.p + s.o_prog),
+                               ln.d_tile_summary.p + 2 * (size_t)s.tile_base[c]),
                    "eval");
                 // pass 2 right behind it on the same stream: all tiles of an activation are in one class, so its counts are final
-                if (want_paths_cls[c]) {
-                    CU(launch_walk(cs, (int)c, tl, n_tiles_cls[c], dacts, ln.d_results.p, reinterpret_cast<const ColOp *>(ln.d_step.p + o_colprog),
-                                   reinterpret_cast<const DpState *>(ln.d_step.p + o_states), reinterpret_cast<const DpEdge *>(ln.d_step.p + o_edges),
-                                   reinterpret_cast<const uint16_t *>(ln.d_step.p + o_costs), reinterpret_cast<const uint32_t *>(ln.d_step.p + o_prog),
-                                   ln.d_tile_summary.p + 2 * (size_t)tile_base[c], ln.d_pathbuf.p, ln.d_qcount.p + 1, (uint32_t)PATH_CAP),
+                if (s.want_paths_cls[c]) {
+                    CU(launch_walk(cs, (int)c, tl, s.n_tiles_cls[c], dacts, ln.d_results.p, reinterpret_cast<const ColOp *>(ln.d_step.p + s.o_colprog),
+                                   reinterpret_cast<const DpState *>(ln.d_step.p + s.o_states), reinterpret_cast<const DpEdge *>(ln.d_step.p + s.o_edges),
+                                   reinterpret_cast<const uint16_t *>(ln.d_step.p + s.o_costs), reinterpret_cast<const uint32_t *>(ln.d_step.p + s.o_prog),
+                                   ln.d_tile_summary.p + 2 * (size_t)s.tile_base[c], ln.d_pathbuf.p, ln.d_qcount.p + 1, (uint32_t)PATH_CAP),
                        "walk");
                     ln.lst.kernel_launches++;
                 }
                 ln.lst.eval_class_launches[c]++;
-                ln.lst.eval_class_tiles[c] += n_tiles_cls[c];
+                ln.lst.eval_class_tiles[c] += s.n_tiles_cls[c];
                 if (c) {
                     ln.lst.kernel_launches++;
                     CU(cudaEventRecord(ln.ev_join[c], cs), "join");
                     CU(cudaStreamWaitEvent(st, ln.ev_join[c], 0), "join wait");
                 }
             }
-            ln.time_kernel(ln.lst, B200_K_EVAL_PATHS, t3, ln.mark(), eval_bytes);
+            ln.time_kernel(ln.lst, B200_K_EVAL_PATHS, t3, ln.mark(), s.eval_bytes);
             CU(cudaMemcpyAsync(ln.h_results, ln.d_results.p, (size_t)res_words * 4, cudaMemcpyDeviceToHost, st), "D2H results");
             CU(cudaMemcpyAsync(ln.h_results + res_words, ln.d_qcount.p, 16, cudaMemcpyDeviceToHost, st), "D2H counters");
         }
@@ -3058,12 +2922,11 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         ln.res_words = res_words;
         ln.qcap = qcap;
         ln.inflight = true;
-        ln.lst.host_ms[3] += ms_since(t_pack);
-        return 1;
-    };
+        return B200_OK;
+    }
 
     // wait for a lane's step, fetch its results and advance its queries
-    auto finish = [&](Lane &ln) -> int {
+    int finish(Lane &ln) {
         auto t_wait = clk::now();
         CU(cudaStreamSynchronize(ln.stream), "step sync");
         ln.inflight = false;
@@ -3138,9 +3001,11 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                 fprintf(stderr, "%s\n", msg.c_str());
             }
             try {
-                PROF(3);
+                ProfScope ps = profile(PROF_ADVANCE);
                 if (pd.node)
                     expand(q, pd.node, out);
+                else if (rule_buckets)
+                    collect_rule_buckets(q);
                 else
                     advance(q);
             } catch (const TooComplex &t) {
@@ -3183,10 +3048,10 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         });
         ln.lst.host_ms[5] += ms_since(t_adv);
         return 0;
-    };
+    }
 
-    auto drive = [&](unsigned dr) -> int {
-        cudaError_t ce = cudaSetDevice(device);
+    int drive(unsigned dr) {
+        cudaError_t ce = cudaSetDevice(eng.device);
         if (ce != cudaSuccess) return cuda_fail(ce, "cudaSetDevice");
         Lane *mine = lanes + dr * lanes_per_driver;
         for (unsigned k = 0; k < lanes_per_driver; k++) {
@@ -3206,76 +3071,68 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             }
             if (!any) return 0;
         }
-    };
-    {
-        // Waves: a driver starts stepping as soon as the terms of ITS queries are derived, while the main thread derives the next
-        // driver's (the derivation sweep is serial device + host work at the head of the call).  B200_WAVES caps the number of waves.
+    }
+    // run driver dr to the end; its outcome becomes its lanes' (fold_lane_stats reports it)
+    void run_driver(unsigned dr) {
+        const int rc = drive(dr);
+        for (unsigned k = 0; k < lanes_per_driver; k++) lanes[dr * lanes_per_driver + k].rc = std::min(lanes[dr * lanes_per_driver + k].rc, rc);
+    }
+    // Waves: a driver starts stepping as soon as the terms of ITS queries are derived, while the main thread derives the next
+    // driver's (the derivation sweep is serial device + host work at the head of the call).  B200_WAVES caps the number of waves.
+    int drive_waves() {
         std::vector<std::thread> drivers;
-        std::vector<int> rcs(n_drivers, 0);
         unsigned n_waves = std::min(2u, n_drivers);
         if (const char *env = getenv("B200_WAVES")) n_waves = (unsigned)std::max(1, std::min((int)n_drivers, atoi(env)));
         int rc_prep = B200_OK;
         for (unsigned wv = 0; wv < n_waves && rc_prep == B200_OK; wv++) {
             const unsigned d0 = n_drivers * wv / n_waves, d1 = n_drivers * (wv + 1) / n_waves;
             const uint32_t lo = lane_lo(d0 * lanes_per_driver), hi = lane_lo(d1 * lanes_per_driver);
-            if (!(s1 && s1->mode == S1Job::RULE)) rc_prep = derive_range(lo, hi);
+            rc_prep = derive_range(lo, hi);
             if (rc_prep != B200_OK) break;
-            if (s1 && s1->mode == S1Job::GRAPH_FROM_TOKENS) {
-                // S1: QueryGraph::from_query with fully computed terms, as an opaque object
-                QState &q = *qs[0];
-                if (q.status != 0) return fail(q.status, q.error);
-                GraphObj *g = new GraphObj(hix);
-                g->ctx.terms = q.ctx.terms;
-                g->ctx.phrases = q.ctx.phrases;
-                g->ctx.phrase_ids = q.ctx.phrase_ids;
-                g->ctx.neg_words = q.ctx.neg_words;
-                g->ctx.neg_phrases = q.ctx.neg_phrases;
-                g->graph = q.graph;
-                s1->graph_out = g;
-                return B200_OK;
-            }
             start_range(lo, hi);
-            kw_derived.store(wv + 1 == n_waves ? KW_DERIVED_ALL : (int)wv + 1, std::memory_order_release);
-            cudaError_t ce = cudaStreamSynchronize(stream);  // row-table memset and derivations visible to the lanes
+            eng.kw_derived.store(wv + 1 == n_waves ? Engine::KW_DERIVED_ALL : (int)wv + 1, std::memory_order_release);
+            cudaError_t ce = cudaStreamSynchronize(eng.stream);  // row-table memset and derivations visible to the lanes
             if (ce != cudaSuccess) {
                 rc_prep = cuda_fail(ce, "sync");
                 break;
             }
-            for (unsigned dr = d0; dr < d1; dr++) drivers.emplace_back([&, dr]() { rcs[dr] = drive(dr); });
+            for (unsigned dr = d0; dr < d1; dr++) drivers.emplace_back([this, dr]() { run_driver(dr); });
         }
         for (auto &t : drivers) t.join();
-        if (rc_prep != B200_OK) return rc_prep;
-        for (unsigned dr = 0; dr < n_drivers; dr++)
-            for (unsigned k = 0; k < lanes_per_driver; k++) lanes[dr * lanes_per_driver + k].rc = std::min(lanes[dr * lanes_per_driver + k].rc, rcs[dr]);
+        return rc_prep;
     }
-    for (unsigned l = 0; l < n_lanes; l++) {  // fold the lanes' statistics (host phases of different lanes overlap in time)
-        const b200_stats &x = lanes[l].lst;
-        stats.kernel_launches += x.kernel_launches;
-        stats.device_steps += x.device_steps;
-        stats.posting_bytes += x.posting_bytes;
-        stats.matrix_bytes += x.matrix_bytes;
-        stats.device_ms += x.device_ms;
-        stats.h2d_bytes += x.h2d_bytes;
-        stats.d2h_bytes += x.d2h_bytes;
-        stats.deferred += x.deferred;
-        for (int k = 0; k < 9; k++) {
-            stats.eval_class_launches[k] += x.eval_class_launches[k];
-            stats.eval_class_tiles[k] += x.eval_class_tiles[k];
+    // fold the lanes' statistics (host phases of different lanes overlap in time); returns the first lane's error
+    int fold_lane_stats() {
+        for (unsigned l = 0; l < n_lanes; l++) {
+            const b200_stats &x = lanes[l].lst;
+            stats.kernel_launches += x.kernel_launches;
+            stats.device_steps += x.device_steps;
+            stats.posting_bytes += x.posting_bytes;
+            stats.matrix_bytes += x.matrix_bytes;
+            stats.device_ms += x.device_ms;
+            stats.h2d_bytes += x.h2d_bytes;
+            stats.d2h_bytes += x.d2h_bytes;
+            stats.deferred += x.deferred;
+            for (int k = 0; k < 9; k++) {
+                stats.eval_class_launches[k] += x.eval_class_launches[k];
+                stats.eval_class_tiles[k] += x.eval_class_tiles[k];
+            }
+            stats.arena_peak_bytes = std::max<uint64_t>(stats.arena_peak_bytes, lanes[l].alloc.peak * n_lanes);
+            for (int k = 0; k < B200_K_COUNT; k++) {
+                stats.kernel_ms[k] += x.kernel_ms[k];
+                stats.kernel_count[k] += x.kernel_count[k];
+                stats.kernel_bytes[k] += x.kernel_bytes[k];
+            }
+            for (int k = 3; k <= 5; k++) stats.host_ms[k] += x.host_ms[k] / n_drivers;  // per driver thread (drivers run concurrently)
         }
-        stats.arena_peak_bytes = std::max<uint64_t>(stats.arena_peak_bytes, lanes[l].alloc.peak * n_lanes);
-        for (int k = 0; k < B200_K_COUNT; k++) {
-            stats.kernel_ms[k] += x.kernel_ms[k];
-            stats.kernel_count[k] += x.kernel_count[k];
-            stats.kernel_bytes[k] += x.kernel_bytes[k];
-        }
-        for (int k = 3; k <= 5; k++) stats.host_ms[k] += x.host_ms[k] / n_drivers;  // per driver thread (drivers run concurrently)
+        for (unsigned l = 0; l < n_lanes; l++)
+            if (lanes[l].rc < 0) return lanes[l].rc;
+        if (r->candidates)
+            for (unsigned l = 0; l < n_lanes; l++) CU(cudaStreamSynchronize(lanes[l].stream), "sync candidates");
+        return B200_OK;
     }
-    for (unsigned l = 0; l < n_lanes; l++)
-        if (lanes[l].rc < 0) return lanes[l].rc;
-    if (r->candidates)
-        for (unsigned l = 0; l < n_lanes; l++) CU(cudaStreamSynchronize(lanes[l].stream), "sync candidates");
     // ---- sort windows of the placeholder searches with sort rules (sort.cu), on the handle's stream
-    {
+    int sort_windows() {
         std::vector<SortDesc> descs;
         std::vector<std::pair<uint32_t, uint32_t>> owner;  // per window: query, first result row
         size_t key_words = 0;
@@ -3294,7 +3151,7 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
             q_elo[i] = elo;
             for (uint32_t lo = elo; lo < ehi; lo += SORT_WINDOW) {
                 SortDesc d{};
-                d.ub = q.d_univ ? q.d_univ : dix.base_ub;
+                d.ub = universe_of(q);
                 d.n_words = hix.n_words64;
                 d.n_levels = L;
                 for (uint32_t l = 0; l < L; l++) {
@@ -3317,23 +3174,23 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
         }
         if (!descs.empty()) {
             const size_t n = descs.size();
-            CU(d_sort_keys.reserve(std::max<size_t>(1, key_words + id_words)), "alloc sort keys");
-            CU(d_sort_info.reserve(2 * n), "alloc sort info");
-            CU(d_sort_desc.reserve(n), "alloc sort windows");
+            CU(eng.d_sort_keys.reserve(std::max<size_t>(1, key_words + id_words)), "alloc sort keys");
+            CU(eng.d_sort_info.reserve(2 * n), "alloc sort info");
+            CU(eng.d_sort_desc.reserve(n), "alloc sort windows");
             for (size_t k = 0; k < n; k++) {
-                descs[k].dst_keys = d_sort_keys.p + (uintptr_t)descs[k].dst_keys;
-                descs[k].dst = d_sort_keys.p + key_words + (uintptr_t)descs[k].dst;
-                descs[k].info = d_sort_info.p + 2 * k;
+                descs[k].dst_keys = eng.d_sort_keys.p + (uintptr_t)descs[k].dst_keys;
+                descs[k].dst = eng.d_sort_keys.p + key_words + (uintptr_t)descs[k].dst;
+                descs[k].info = eng.d_sort_info.p + 2 * k;
             }
-            CU(cudaMemcpyAsync(d_sort_desc.p, descs.data(), n * sizeof(SortDesc), cudaMemcpyHostToDevice, stream), "H2D sort windows");
-            const size_t m0 = mark();
-            CU(launch_sort_window(stream, d_sort_desc.p, (uint32_t)n), "sort_window");
-            time_kernel(B200_K_SORT, m0, mark(), 0);
+            CU(cudaMemcpyAsync(eng.d_sort_desc.p, descs.data(), n * sizeof(SortDesc), cudaMemcpyHostToDevice, eng.stream), "H2D sort windows");
+            const size_t m0 = eng.mark();
+            CU(launch_sort_window(eng.stream, eng.d_sort_desc.p, (uint32_t)n), "sort_window");
+            eng.time_kernel(B200_K_SORT, m0, eng.mark(), 0);
             std::vector<uint32_t> keys(key_words + id_words), info(2 * n);
-            CU(cudaMemcpyAsync(keys.data(), d_sort_keys.p, (key_words + id_words) * 4, cudaMemcpyDeviceToHost, stream), "D2H sort keys");
-            CU(cudaMemcpyAsync(info.data(), d_sort_info.p, 2 * n * 4, cudaMemcpyDeviceToHost, stream), "D2H sort info");
-            CU(cudaStreamSynchronize(stream), "sync sort");
-            resolve_timers();
+            CU(cudaMemcpyAsync(keys.data(), eng.d_sort_keys.p, (key_words + id_words) * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H sort keys");
+            CU(cudaMemcpyAsync(info.data(), eng.d_sort_info.p, 2 * n * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H sort info");
+            CU(cudaStreamSynchronize(eng.stream), "sync sort");
+            eng.resolve_timers();
             stats.h2d_bytes += n * sizeof(SortDesc);
             stats.d2h_bytes += (key_words + id_words) * 4 + 2 * n * 4;
             for (size_t k = 0; k < n; k++) {
@@ -3353,8 +3210,8 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                 const SortDesc &d0 = descs[q_first[i]];
                 const uint32_t L = d0.n_levels, elo = q_elo[i];
                 const uint32_t n_ext = (uint32_t)std::min<uint64_t>(q.univ_count, (uint64_t)q.sort_hi + 1) - elo;
-                const uint32_t *ids = keys.data() + key_words + ((uintptr_t)d0.dst - (uintptr_t)(d_sort_keys.p + key_words)) / 4;
-                const uint32_t *kp = keys.data() + ((uintptr_t)d0.dst_keys - (uintptr_t)d_sort_keys.p) / 4;
+                const uint32_t *ids = keys.data() + key_words + ((uintptr_t)d0.dst - (uintptr_t)(eng.d_sort_keys.p + key_words)) / 4;
+                const uint32_t *kp = keys.data() + ((uintptr_t)d0.dst_keys - (uintptr_t)eng.d_sort_keys.p) / 4;
                 auto shares = [&](uint32_t a, uint32_t b, uint32_t n_keys) {  // keys [0, n_keys) of ext rows a and b agree
                     for (uint32_t l = 0; l < n_keys; l++)
                         if (kp[(size_t)a * L + l] != kp[(size_t)b * L + l]) return false;
@@ -3385,7 +3242,7 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                     std::vector<EScore> &sc = q.scores[j];
                     sc.clear();
                     for (uint32_t l = 0; l < n_sc; l++) {
-                        const QState::SortRule &rule = q.sort_rules[l];
+                        const SortRule &rule = q.sort_rules[l];
                         const uint32_t key = kp[(size_t)e * L + l];
                         auto it = hix.sort_fields.find(rule.fid);
                         bool is_string = false;
@@ -3396,88 +3253,178 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
                 }
             }
         }
+        return B200_OK;
     }
-    // ---- outputs
-    t_ph = clk::now();
-    std::vector<uint32_t> out_ids((size_t)NQ * std::max(1u, length));
-    CU(cudaMemcpyAsync(out_ids.data(), d_docids_out.p, out_ids.size() * 4, cudaMemcpyDeviceToHost, stream), "D2H docids");
-    stats.d2h_bytes += out_ids.size() * 4;
-    stats.h2d_bytes += (size_t)b->lemma_off[b->token_begin[NQ]] + (size_t)b->token_begin[NQ] * 5 + (size_t)NQ * 4;
-    CU(cudaStreamSynchronize(stream), "sync");
-    for (uint32_t i = 0; i < NQ; i++) {
-        QState &q = *qs[i];
-        if (r->status) r->status[i] = q.status;
-        if (q.status != 0) {
-            r->n_hits[i] = 0;
-            if (r->n_candidates) r->n_candidates[i] = 0;
-            last_error = q.error;
-            continue;
-        }
-        r->n_hits[i] = q.n_results;
-        if (q.sort_pending)
-            for (uint32_t k = 0; k < q.n_results; k++) out_ids[(size_t)i * std::max(1u, length) + k] = q.sort_ids[k];
-        if (r->n_candidates) r->n_candidates[i] = q.n_candidates;
-        if (r->degraded) r->degraded[i] = q.degraded ? 1 : 0;
-        if (r->used_negative_operator) r->used_negative_operator[i] = q.used_negative ? 1 : 0;
-        for (uint32_t k = 0; k < q.n_results; k++) {
-            r->docids[(size_t)i * limit + k] = out_ids[(size_t)i * std::max(1u, length) + k];
-            if (r->n_scores) {
-                const auto &sc = q.scores[k];
-                size_t ns = std::min<size_t>(sc.size(), B200_MAX_SCORES);
-                r->n_scores[(size_t)i * limit + k] = (uint8_t)ns;
-                for (size_t s = 0; s < ns; s++) {
-                    size_t at = ((size_t)i * limit + k) * B200_MAX_SCORES + s;
-                    r->score_kind[at] = sc[s].kind;
-                    r->score_rank[at] = sc[s].rank;
-                    r->score_max[at] = sc[s].max_rank;
-                    r->score_sim[at] = sc[s].sim;
+    int write_results() {
+        std::vector<uint32_t> out_ids((size_t)NQ * std::max(1u, length));
+        CU(cudaMemcpyAsync(out_ids.data(), eng.d_docids_out.p, out_ids.size() * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H docids");
+        stats.d2h_bytes += out_ids.size() * 4;
+        stats.h2d_bytes += (size_t)b->lemma_off[b->token_begin[NQ]] + (size_t)b->token_begin[NQ] * 5 + (size_t)NQ * 4;
+        CU(cudaStreamSynchronize(eng.stream), "sync");
+        for (uint32_t i = 0; i < NQ; i++) {
+            QState &q = *qs[i];
+            if (r->status) r->status[i] = q.status;
+            if (q.status != 0) {
+                r->n_hits[i] = 0;
+                if (r->n_candidates) r->n_candidates[i] = 0;
+                eng.last_error = q.error;
+                continue;
+            }
+            r->n_hits[i] = q.n_results;
+            if (q.sort_pending)
+                for (uint32_t k = 0; k < q.n_results; k++) out_ids[(size_t)i * std::max(1u, length) + k] = q.sort_ids[k];
+            if (r->n_candidates) r->n_candidates[i] = q.n_candidates;
+            if (r->degraded) r->degraded[i] = q.degraded ? 1 : 0;
+            if (r->used_negative_operator) r->used_negative_operator[i] = q.used_negative ? 1 : 0;
+            for (uint32_t k = 0; k < q.n_results; k++) {
+                r->docids[(size_t)i * length + k] = out_ids[(size_t)i * std::max(1u, length) + k];
+                if (r->n_scores) {
+                    const auto &sc = q.scores[k];
+                    size_t ns = std::min<size_t>(sc.size(), B200_MAX_SCORES);
+                    r->n_scores[(size_t)i * length + k] = (uint8_t)ns;
+                    for (size_t s = 0; s < ns; s++) {
+                        size_t at = ((size_t)i * length + k) * B200_MAX_SCORES + s;
+                        r->score_kind[at] = sc[s].kind;
+                        r->score_rank[at] = sc[s].rank;
+                        r->score_max[at] = sc[s].max_rank;
+                        r->score_sim[at] = sc[s].sim;
+                    }
                 }
             }
         }
+        return B200_OK;
     }
-    if (work_hist) {
-        static const char *ucls[4] = {"ld<128", "ld<4096", "ld<65536", "ld>=65536"};
-        static const char *kinds[10] = {"words", "typo", "proximity", "fid", "position", "exactness", "exact_attr", "resolve", "freq", "?"};
-        for (int u = 0; u < 4; u++) {
-            fprintf(stderr, "[b200 work] scatter lists, universe %s (pair probes %llu):\n", ucls[u], (unsigned long long)work_hist->probes[u]);
-            for (int c = 0; c < 33; c++)
-                if (work_hist->lists[u][c][0])
-                    fprintf(stderr, "    %s%-2d lists %9llu  bytes %8.1f MB\n", c == 32 ? "dense " : "card<=2^", c == 32 ? 0 : c,
-                            (unsigned long long)work_hist->lists[u][c][0], work_hist->lists[u][c][1] / 1e6);
+    // B200_WORK_HIST / B200_PROFILE reports of the batch
+    void debug_reports() {
+        if (work_hist) {
+            static const char *ucls[4] = {"ld<128", "ld<4096", "ld<65536", "ld>=65536"};
+            static const char *kinds[10] = {"words", "typo", "proximity", "fid", "position", "exactness", "exact_attr", "resolve", "freq", "?"};
+            for (int u = 0; u < 4; u++) {
+                fprintf(stderr, "[b200 work] scatter lists, universe %s (pair probes %llu):\n", ucls[u], (unsigned long long)work_hist->probes[u]);
+                for (int c = 0; c < 33; c++)
+                    if (work_hist->lists[u][c][0])
+                        fprintf(stderr, "    %s%-2d lists %9llu  bytes %8.1f MB\n", c == 32 ? "dense " : "card<=2^", c == 32 ? 0 : c,
+                                (unsigned long long)work_hist->lists[u][c][0], work_hist->lists[u][c][1] / 1e6);
+            }
+            for (int k = 0; k < 10; k++)
+                for (int u = 0; u < 4; u++)
+                    if (work_hist->eval[k][u][0])
+                        fprintf(stderr, "[b200 work] eval %-10s %-10s acts %7llu rows %10llu row*ops %12llu row*cols %11llu\n", kinds[k], ucls[u],
+                                (unsigned long long)work_hist->eval[k][u][0], (unsigned long long)work_hist->eval[k][u][1],
+                                (unsigned long long)work_hist->eval[k][u][2], (unsigned long long)work_hist->eval[k][u][3]);
         }
-        for (int k = 0; k < 10; k++)
-            for (int u = 0; u < 4; u++)
-                if (work_hist->eval[k][u][0])
-                    fprintf(stderr, "[b200 work] eval %-10s %-10s acts %7llu rows %10llu row*ops %12llu row*cols %11llu\n", kinds[k], ucls[u],
-                            (unsigned long long)work_hist->eval[k][u][0], (unsigned long long)work_hist->eval[k][u][1],
-                            (unsigned long long)work_hist->eval[k][u][2], (unsigned long long)work_hist->eval[k][u][3]);
+        if (prof)
+            fprintf(stderr, "[b200 profile] thread-ms: build_from_paths %.2f  prepare_graph_rule %.2f  request_activation %.2f  advance(total) %.2f\n",
+                    prof_ns[0] / 1e6, prof_ns[1] / 1e6, prof_ns[2] / 1e6, prof_ns[3] / 1e6);
     }
-    if (prof)
-        fprintf(stderr, "[b200 profile] thread-ms: build_from_paths %.2f  prepare_graph_rule %.2f  request_activation %.2f  advance(total) %.2f\n",
-                prof_ns[0] / 1e6, prof_ns[1] / 1e6, prof_ns[2] / 1e6, prof_ns[3] / 1e6);
-#undef PROF
     // tear the per-query state down off the critical path
-    for (auto &t : reapers)
-        if (t.joinable()) t.join();
-    reapers.clear();
-    {
-        const size_t n_reapers = 4, per = (qs.size() + n_reapers - 1) / n_reapers;
-        for (size_t r0 = 0; r0 < qs.size(); r0 += std::max<size_t>(1, per)) {
-            auto *dead = new std::vector<std::unique_ptr<QState>>();
-            for (size_t i = r0; i < std::min(qs.size(), r0 + per); i++) dead->push_back(std::move(qs[i]));
-            reapers.emplace_back([dead]() { delete dead; });
+    void reap() {
+        for (auto &t : eng.reapers)
+            if (t.joinable()) t.join();
+        eng.reapers.clear();
+        {
+            const size_t n_reapers = 4, per = (qs.size() + n_reapers - 1) / n_reapers;
+            for (size_t r0 = 0; r0 < qs.size(); r0 += std::max<size_t>(1, per)) {
+                auto *dead = new std::vector<std::unique_ptr<QState>>();
+                for (size_t i = r0; i < std::min(qs.size(), r0 + per); i++) dead->push_back(std::move(qs[i]));
+                eng.reapers.emplace_back([dead]() { delete dead; });
+            }
         }
     }
-    stats.host_ms[6] += ms_since(t_ph);
-    stats.host_ms[7] += ms_since(t_total);
-    return B200_OK;
+    // after the step loop: statistics, sort windows, results and reports; the per-query state is freed in the background
+    int finish_batch() {
+        int rc = fold_lane_stats();
+        if (rc == B200_OK) rc = sort_windows();
+        if (rc != B200_OK) return rc;
+        const auto t_out = clk::now();
+        if ((rc = write_results()) != B200_OK) return rc;
+        debug_reports();
+        reap();
+        stats.host_ms[6] += ms_since(t_out);
+        stats.host_ms[7] += ms_since(t_total);
+        return B200_OK;
+    }
+};
+
+}  // namespace
+
+// The sort rules of query qi (search/new/mod.rs:351-416, 651-716): the `Sort` criterion expands to the query's `sort` list at its
+// position, once; Asc(f) / Desc(f) criteria add one rule each; a field sorted earlier in the list is skipped.  Sort is built for
+// placeholder keyword searches; every other search with sort rules is refused with B200_ERR_UNSUPPORTED rather than answered without
+// them.  Returns B200_OK with the rules in `out`, or the code the query fails with and `why`.
+int Engine::sort_rules(const b200_query_batch *b, uint32_t qi, bool semantic, bool placeholder, std::vector<SortRule> &out, const char *&why) const {
+    bool has_sort_criterion = false, has_custom = false;
+    for (int c : hix.settings.criteria) {
+        has_sort_criterion |= c == B200_C_SORT;
+        has_custom |= (c & 0x30000) != 0;
+    }
+    const uint32_t s0 = b->sort_begin ? b->sort_begin[qi] : 0, s1 = b->sort_begin ? b->sort_begin[qi + 1] : 0;
+    if (s1 > s0 && !has_sort_criterion) {  // check_sort_criteria (search/new/mod.rs:998-1016)
+        why = "SortRankingRuleMissing: a sort list was given but the ranking rules do not contain `sort`";
+        return B200_ERR_INVALID;
+    }
+    if (semantic) {  // get_ranking_rules_for_vector (search/new/mod.rs:419-508)
+        if (s1 == s0 && !has_custom) return B200_OK;
+        why = "sort rules in a semantic search (sort list or Asc/Desc criteria) are not built";
+        return B200_ERR_UNSUPPORTED;
+    }
+    if (s1 > s0 && (!b->sort_fid || !b->sort_asc)) {
+        why = "sort_begin without sort_fid / sort_asc";
+        return B200_ERR_INVALID;
+    }
+    std::vector<SortRule> sr;
+    std::vector<uint16_t> sorted;
+    bool sort_done = false;
+    auto add = [&](uint16_t fid, bool asc) {
+        // 0xFFFF stands for every field absent from the fields map: its entries are never "already sorted" (the caller,
+        // which sees the names, drops a repeated absent name)
+        if (fid != 0xFFFF && std::find(sorted.begin(), sorted.end(), fid) != sorted.end()) return;
+        sorted.push_back(fid);
+        sr.push_back(SortRule{fid, asc});
+    };
+    for (int c : hix.settings.criteria) {
+        if (c == B200_C_SORT && !sort_done) {
+            sort_done = true;
+            for (uint32_t k = s0; k < s1; k++) add(b->sort_fid[k], b->sort_asc[k] != 0);
+        } else if (c & 0x10000)
+            add((uint16_t)(c & 0xffff), true);
+        else if (c & 0x20000)
+            add((uint16_t)(c & 0xffff), false);
+    }
+    if (sr.empty()) return B200_OK;
+    if (b->mode != 0)
+        why = "sort in a semantic or hybrid search (needs the ScoreValue::Sort comparator of hybrid.rs)";
+    else if (!placeholder)
+        why = "sort rule in a search with query terms (sort is built for placeholder searches)";
+    else if (sr.size() > B200_MAX_SCORES)
+        why = "more than B200_MAX_SCORES sort rules";
+    else if (b->stop_after >= 0)
+        why = "stop_after together with a sort rule (the sort window is one device step; its polls are not counted)";
+    else {
+        out = std::move(sr);
+        return B200_OK;
+    }
+    return B200_ERR_UNSUPPORTED;
+}
+
+int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t offset, uint32_t limit, int scoring) {
+    CU(cudaSetDevice(device), "cudaSetDevice");
+    AffinityScope on_gpu_socket(affinity);  // before any thread of this call is created
+    KeywordBatch kb(*this, b, r, offset, limit, scoring);
+    kb.parse();
+    kb.resolve_sort_rules();
+    int rc = kb.stage_universes();
+    if (rc == B200_OK) rc = kb.setup_lanes();
+    if (rc == B200_OK) rc = kb.drive_waves();
+    if (rc == B200_OK) rc = kb.finish_batch();
+    return rc;
 }
 
 // ================================================================================================ S1: the RankingRule seam
 void free_graph(GraphObj *g) { delete g; }
 
 struct Engine::RuleRun {
-    std::vector<S1Job::Bucket> buckets;
+    std::vector<RuleBucket> buckets;
     size_t cursor = 0;
     ~RuleRun() {
         for (auto &b : buckets) delete b.child;
@@ -3489,12 +3436,20 @@ struct Engine::RuleRun {
 int Engine::graph_from_tokens(const b200_query_batch *one, GraphObj **out) {
     *out = nullptr;
     if (one->n_queries != 1) return fail(B200_ERR_INVALID, "graph_from_tokens takes exactly one query");
-    S1Job job;
-    job.mode = S1Job::GRAPH_FROM_TOKENS;
+    CU(cudaSetDevice(device), "cudaSetDevice");
+    AffinityScope on_gpu_socket(affinity);
     b200_results none{};
-    int rc = keyword_batch(one, &none, 0, 1, 0, &job);
+    KeywordBatch kb(*this, one, &none, 0, 1, 0);
+    kb.parse();
+    // Sort rules are resolved as in a search, so on an index whose criteria hold Asc/Desc a query with terms is refused with
+    // B200_ERR_UNSUPPORTED (sort is built for placeholder searches only).
+    kb.resolve_sort_rules();
+    int rc = kb.stage_universes();
+    if (rc == B200_OK) rc = kb.derive_range(0, 1);
     if (rc != B200_OK) return rc;
-    *out = job.graph_out;
+    const QState &q = *kb.qs[0];
+    if (q.status != 0) return fail(q.status, q.error);
+    *out = new GraphObj(q.ctx, q.graph);
     return B200_OK;
 }
 
@@ -3504,10 +3459,6 @@ int Engine::rule_start(int rule_kind, int tms, const GraphObj *query, const uint
     *out = nullptr;
     static const int kinds[7] = {RK_WORDS, RK_TYPO, RK_PROXIMITY, RK_FID, RK_POSITION, RK_EXACT_ATTRIBUTE, RK_EXACTNESS};
     if (rule_kind < 0 || rule_kind > 6 || !query) return fail(B200_ERR_INVALID, "rule_start: unknown rule kind or null query graph");
-    S1Job job;
-    job.mode = S1Job::RULE;
-    job.graph_in = query;
-    job.rule_kind = kinds[rule_kind];
     static const uint32_t zeros[2] = {0, 0};
     static const uint8_t kind0[1] = {0};
     b200_query_batch b{};
@@ -3533,18 +3484,28 @@ int Engine::rule_start(int rule_kind, int tms, const GraphObj *query, const uint
     r.n_hits = n_hits;
     r.status = status;
     r.n_candidates = n_cand;
-    int rc = keyword_batch(&b, &r, 0, 1, 0, &job);
-    if (rc != B200_OK) {
-        for (auto &bk : job.buckets) delete bk.child;
-        return rc;
+    CU(cudaSetDevice(device), "cudaSetDevice");
+    AffinityScope on_gpu_socket(affinity);
+    std::unique_ptr<RuleRun> run(new RuleRun());
+    KeywordBatch kb(*this, &b, &r, 0, 1, 0);
+    kb.rule_buckets = &run->buckets;
+    QState &q = *kb.qs[0];
+    static_cast<QTerms &>(q.ctx) = query->ctx;
+    q.graph = query->graph;
+    // Sort rules are resolved as in a search.  The query graph is never parsed here, so it is never a placeholder: on an index whose
+    // criteria hold Asc/Desc every rule_start is refused with B200_ERR_UNSUPPORTED.
+    kb.resolve_sort_rules();
+    int rc = kb.stage_universes();
+    if (rc == B200_OK) rc = kb.setup_lanes();
+    if (rc == B200_OK) {
+        if (!q.done) kb.start_rule(q, kinds[rule_kind]);
+        CU(cudaStreamSynchronize(stream), "sync");  // row-table memset visible to the lane
+        kb.run_driver(0);
+        rc = kb.finish_batch();
     }
-    if (status[0] != 0) {
-        for (auto &bk : job.buckets) delete bk.child;
-        return fail(status[0], last_error);
-    }
-    RuleRun *run = new RuleRun();
-    run->buckets = std::move(job.buckets);
-    *out = run;
+    if (rc != B200_OK) return rc;
+    if (status[0] != 0) return fail(status[0], last_error);
+    *out = run.release();
     return B200_OK;
 }
 
@@ -3554,7 +3515,7 @@ namespace b200 {
 int rule_next_impl(Engine::RuleRun *run, uint64_t n_words64, const uint64_t *universe, uint64_t *out_bitmap, uint64_t n_words, uint32_t *rank,
                    uint32_t *max_rank, GraphObj **out_query) {
     if (run->cursor >= run->buckets.size()) return 1;
-    S1Job::Bucket &b = run->buckets[run->cursor++];
+    RuleBucket &b = run->buckets[run->cursor++];
     if (rank) *rank = b.rank;
     if (max_rank) *max_rank = b.max_rank;
     if (out_bitmap)

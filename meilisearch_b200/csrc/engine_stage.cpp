@@ -92,11 +92,6 @@ Engine::~Engine() {
         for (auto p : kv.second.d_key)
             if (p) cudaFree(p);
     for (auto &ln : lanes) ln.release();
-    d_step.release();
-    d_results.release();
-    d_queue.release();
-    d_qcount.release();
-    d_pathbuf.release();
     d_docids_out.release();
     d_sort_desc.release();
     d_sort_keys.release();
@@ -110,8 +105,6 @@ Engine::~Engine() {
     d_vsel_ids.release();
     d_vsel_n.release();
     d_cand.release();
-    if (h_step) cudaFreeHost(h_step);
-    if (h_results) cudaFreeHost(h_results);
     for (auto e : ev_pool) cudaEventDestroy(e);
     if (sc.comm && sc.comm_destroy) sc.comm_destroy(sc.comm);
     d_gather_ids.release();
@@ -119,8 +112,6 @@ Engine::~Engine() {
     d_gather_n.release();
     for (auto e : vt.ev_pool) cudaEventDestroy(e);
     if (vt.stream) cudaStreamDestroy(vt.stream);
-    if (ev0) cudaEventDestroy(ev0);
-    if (ev1) cudaEventDestroy(ev1);
     if (stream) cudaStreamDestroy(stream);
 }
 
@@ -461,7 +452,6 @@ int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t l
     std::vector<float> qinv(chunk);
     std::vector<float> sel_d((size_t)chunk * (limit + tie_cap));
     std::vector<uint32_t> sel_i((size_t)chunk * (limit + tie_cap)), sel_n((size_t)chunk * 2);
-    float total_ms = 0;
     for (uint32_t q0 = 0; q0 < n_q; q0 += chunk) {
         uint32_t nq = std::min(chunk, n_q - q0);
         for (uint32_t q = 0; q < nq; q++) {
@@ -523,7 +513,6 @@ int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t l
             }
         }
     }
-    (void)total_ms;
     return B200_OK;
 }
 
