@@ -4,7 +4,8 @@ Key: u16 BE fid | u8 level | bound (OrderedF64Codec, heed_codec/facet/ordered_f6
 value: FacetGroupValueCodec = u8 size | CBO roaring (heed_codec/facet/mod.rs).  Level-0 entries hold one value each; levels >= 1
 group FACET_GROUP_SIZE entries of the level below (left bound = the first one's) as the reference's incremental indexer does, so
 that readers which must ignore them see them.  JSON documents go through milli's extraction rules: arrays are flattened, `null`,
-objects and the empty string get no facet, booleans become the strings "true" / "false", strings are normalised (lib.rs:442)."""
+objects and the empty string get no facet, booleans become the strings "true" / "false", strings are normalised (lib.rs:442).
+`_geo` objects become the number facets `_geo.lat` / `_geo.lng` (update/new/extract/faceted/facet_document.rs:82-99)."""
 from __future__ import annotations
 
 import struct
@@ -95,7 +96,15 @@ class FacetImage:
             self.numbers.setdefault(f, {}).setdefault(float(value), []).append(docid)
 
     def add_json(self, docid, name, value):
-        """a JSON field value through milli's facet extraction: arrays flattened; null / objects / "" give nothing"""
+        """a JSON field value through milli's facet extraction: arrays flattened; null / objects / "" give nothing; `_geo`
+        ({"lat": .., "lng": ..}, numbers or numeric strings) gives the number facets `_geo.lat` / `_geo.lng`"""
+        if name == "_geo":
+            if value is None:
+                return
+            lat, lng = (float(value[k]) for k in ("lat", "lng"))  # extract_geo_coordinates: both, as f64 (else the document is refused)
+            self.add_facet(docid, "_geo.lat", lat)
+            self.add_facet(docid, "_geo.lng", lng)
+            return
         self.fid(name)
         if isinstance(value, list):
             for v in value:
@@ -131,6 +140,36 @@ class FacetImage:
             self._bulk("tags", sel[~is_num], strs[~is_num], numbers=False)
         return self
 
+    def add_synthetic_geo(self, n_docs, seed=0x6E0, with_geo=0.9):
+        """seeded `_geo` points for the GeoSort tests: clusters around a few cities, exact duplicates, runs of points less than 1 m
+        apart (chains of the 1 m error margin), points at distances sharing a floor metre, antipodes, the +/-180 degree seam, and
+        documents without `_geo` (1 - with_geo of them)"""
+        rng = np.random.default_rng(seed)
+        docs = np.arange(n_docs)
+        has = rng.random(n_docs) < with_geo
+        kind = rng.integers(0, 6, n_docs)
+        centers = np.array([[48.85, 2.35], [40.71, -74.0], [-33.86, 151.21], [35.68, 139.69], [0.0, 179.99], [-48.85, -177.65]])
+        c = centers[rng.integers(0, len(centers), n_docs)]
+        lat = np.clip(c[:, 0] + rng.normal(0, 0.5, n_docs), -90, 90)
+        lng = c[:, 1] + rng.normal(0, 0.5, n_docs)
+        lng = (lng + 180.0) % 360.0 - 180.0
+        # kind 1: exact duplicates of a handful of points; 2: chains of points ~0.4 m apart; 3: uniform over the sphere;
+        # 4: round coordinates (many equal floor metres); 5: cluster (kept)
+        dup = rng.integers(0, 40, n_docs)
+        lat = np.where(kind == 1, 10.0 + dup * 0.001, lat)
+        lng = np.where(kind == 1, 20.0, lng)
+        step = docs * 3.6e-6  # about 0.4 m of latitude per document
+        lat = np.where(kind == 2, 45.0 + (step % 0.01), lat)
+        lng = np.where(kind == 2, 7.0, lng)
+        u = rng.random(n_docs)
+        lat = np.where(kind == 3, np.degrees(np.arcsin(2 * u - 1)), lat)
+        lng = np.where(kind == 3, rng.uniform(-180, 180, n_docs), lng)
+        lat = np.where(kind == 4, np.round(lat, 1), lat)
+        lng = np.where(kind == 4, np.round(lng, 1), lng)
+        self._bulk("_geo.lat", docs[has], lat[has], numbers=True)
+        self._bulk("_geo.lng", docs[has], lng[has], numbers=True)
+        return self
+
     def _bulk(self, name, docids, values, numbers):
         f = self.fid(name)
         tab = (self.numbers if numbers else self.strings).setdefault(f, {})
@@ -163,3 +202,19 @@ class FacetImage:
                 lv += 1
         out.sort(key=lambda e: e[0])
         return out
+
+
+def geo_points(facets, lat_fid, lng_fid):
+    """docid -> (lat, lng) as geo_value reads it (documents/geo_sort.rs:252-277): per coordinate the smallest number value, else the
+    bytewise-smallest string value parsed as f64; documents with neither coordinate are left out"""
+    out = [{}, {}]
+    for c, fid in enumerate((lat_fid, lng_fid)):
+        for v in sorted(facets.numbers.get(fid, {})):
+            for d in facets.numbers[fid][v]:
+                out[c].setdefault(d, v)
+        for v in sorted(facets.strings.get(fid, {}), key=lambda x: x.encode()):
+            for d in facets.strings[fid][v]:
+                out[c].setdefault(d, float(v))
+    if set(out[0]) != set(out[1]):
+        raise ValueError("a document has one geo coordinate without the other")
+    return {d: (out[0][d], out[1][d]) for d in out[0]}

@@ -20,7 +20,7 @@ extern "C" {
 #define B200_ERR_NO_DEVICE (-1)   /* no CUDA device / driver (the product never falls back to the CPU) */
 #define B200_ERR_CUDA (-2)        /* a CUDA call failed; see b200_last_error */
 #define B200_ERR_INVALID (-3)     /* bad argument */
-#define B200_ERR_UNSUPPORTED (-4) /* query feature outside the implemented scope (geo, distinct, more than 12 terms, ...) */
+#define B200_ERR_UNSUPPORTED (-4) /* query feature outside the implemented scope (distinct, more than 12 terms, ...) */
 #define B200_ERR_CAPACITY (-5)    /* a device work queue / arena overflowed */
 #define B200_ERR_STATE (-6)       /* call order (e.g. search before b200_stage_finish) */
 
@@ -88,6 +88,14 @@ int b200_stage_settings(b200_index *, const b200_settings *);
  * parse_query.rs:277-285): entry i maps the word sequence from_words[i] to the word sequence to_words[i], both already
  * tokenised and joined by single spaces.  Several entries may share the same `from`.  Replaces any previous set. */
 int b200_stage_synonyms(b200_index *, uint32_t n, const char *const *from_words, const char *const *to_words);
+/* The GeoSort rule's fields (search/new/geo_sort.rs): the fids of `_geo.lat` and `_geo.lng` in the facet databases.  Indexing writes
+ * them as number facets (update/new/extract/faceted/facet_document.rs:82-99); b200_stage_finish reads each document's point from
+ * their level-0 entries in facet_id_f64_docids (the smallest value when there are several, as geo_value's prefix iteration takes,
+ * documents/geo_sort.rs:252-277), else from facet_id_string_docids parsed as f64.  The geo documents (geo_faceted_documents_ids)
+ * are those with a point.  A document with only one of the two coordinates, or an unparsable string one, makes
+ * b200_stage_finish fail with B200_ERR_INVALID (the reference panics).  Without this call no document is geo: every GeoSort rule
+ * returns one Null bucket.  Must precede b200_stage_finish. */
+int b200_stage_geo_fields(b200_index *, uint16_t lat_fid, uint16_t lng_fid);
 /* Uploads everything to HBM and builds the device directories.  Must follow the stage_* calls. */
 int b200_stage_finish(b200_index *);
 /* Replaces the arroy/hannoy item nodes read by VectorStore (crates/milli/src/vector/store.rs:1427-1434):
@@ -184,27 +192,41 @@ typedef struct {
     int32_t has_ranking_score_threshold;
     double ranking_score_threshold;
     /* Search::sort_criteria (search/mod.rs:160): the `sort` list of query i is entries [sort_begin[i], sort_begin[i+1]) of
-     * sort_fid / sort_asc; sort_begin NULL = no `sort` anywhere.  sort_fid: the field's id in the facet databases, 0xFFFF for a
-     * field absent from the fields map (it sorts nothing: every document lands in the Null bucket).  Rules on a field already
+     * sort_fid / sort_asc / sort_geo; sort_begin NULL = no `sort` anywhere.  sort_fid: the field's id in the facet databases, 0xFFFF
+     * for a field absent from the fields map (it sorts nothing: every document lands in the Null bucket).  Rules on a field already
      * sorted earlier in the rule list are skipped by fid; 0xFFFF entries are never skipped, so the caller, which sees the names,
      * leaves out an absent field whose name is already sorted (milli deduplicates by name); sort_asc: 1 Asc, 0 Desc.
-     * The sortable-attributes check and `_geoPoint` stay with the caller.  A non-empty list while the criteria lack `sort`
+     * sort_geo (NULL = none): 1 marks a `_geoPoint(lat, lng)` entry, whose point is sort_geo_point[2 k], [2 k + 1] and whose sort_fid
+     * is ignored.  Each one adds a GeoSort rule; geo entries are never deduplicated (resolve_sort_criteria, search/new/mod.rs:651-716).
+     * The sortable-attributes check stays with the caller.  A non-empty list while the criteria lack `sort`
      * (SortRankingRuleMissing, search/new/mod.rs:998-1040) is B200_ERR_INVALID for that query, in every mode.  Sort rules are
      * implemented for placeholder searches of mode 0 only (no positive or negative query term: the rule stack is the sort rules
-     * alone, search/new/mod.rs:353-416).  B200_ERR_UNSUPPORTED for that query, never an answer without its sort rules: a sort rule
-     * (from the list or from Asc/Desc criteria) in a search with query terms or with negative terms only, in a semantic or hybrid
-     * search, more than B200_MAX_SCORES sort rules, `stop_after` together with a sort rule. */
+     * alone, search/new/mod.rs:353-416), and a GeoSort rule only as the first rule of that stack.  B200_ERR_UNSUPPORTED for that
+     * query, never an answer without its sort rules: a sort rule (from the list or from Asc/Desc criteria) in a search with query
+     * terms or with negative terms only, in a semantic or hybrid search, more than B200_MAX_SCORES sort rules, `stop_after`
+     * together with a sort rule, a GeoSort rule after the first rule. */
     const uint32_t *sort_begin;
     const uint16_t *sort_fid;
     const uint8_t *sort_asc;
+    const uint8_t *sort_geo;
+    const double *sort_geo_point;
+    /* Search::geo_sort_strategy / geo_max_bucket_size (search/mod.rs:190-198, documents/geo_sort.rs:12-63): geo_strategy 0
+     * Dynamic(geo_cache_size), 1 AlwaysIterative(geo_cache_size), 2 AlwaysRtree(geo_cache_size); geo_cache_size 0 = 1000;
+     * geo_max_bucket_size 0 = 1000.  The distance error margin is the reference's 1.0 m. */
+    int32_t geo_strategy;
+    uint32_t geo_cache_size;
+    uint64_t geo_max_bucket_size;
 } b200_query_batch;
 #define B200_MAX_SCORES 12
 /* score kinds: ScoreDetails variants (score_details.rs:9-32) */
 enum b200_score_kind { B200_S_WORDS = 0, B200_S_TYPO = 1, B200_S_PROXIMITY = 2, B200_S_FID = 3, B200_S_POSITION = 4,
-                       B200_S_EXACT_ATTRIBUTE = 5, B200_S_EXACT_WORDS = 6, B200_S_VECTOR = 7, B200_S_SKIPPED = 8, B200_S_SORT = 9 };
+                       B200_S_EXACT_ATTRIBUTE = 5, B200_S_EXACT_WORDS = 6, B200_S_VECTOR = 7, B200_S_SKIPPED = 8, B200_S_SORT = 9,
+                       B200_S_GEO_SORT = 10 };
 /* B200_S_SORT (ScoreDetails::Sort, score_details.rs): score_max = fid << 2 | ascending << 1 | is_string; score_rank = position of
  * the bucket's value among the staged level-0 keys of its database (facet_id_f64_docids when is_string = 0, else
- * facet_id_string_docids), 0xFFFFFFFF for the Null bucket (no value).  Sort has no Rank: global scores ignore it. */
+ * facet_id_string_docids), 0xFFFFFFFF for the Null bucket (no value).  Sort has no Rank: global scores ignore it.
+ * B200_S_GEO_SORT (ScoreDetails::GeoSort): score_rank = docid of the bucket's first point (its `value` is that document's point),
+ * 0xFFFFFFFF for the Null bucket (None); score_max = ascending << 1; the target point is the query's.  No Rank either. */
 typedef struct {                  /* SearchResult (search/mod.rs:526-535), flattened; all caller-allocated */
     uint32_t *docids;             /* n_queries x limit      documents_ids */
     uint32_t *n_hits;             /* n_queries */
@@ -252,7 +274,8 @@ void b200_rule_end(b200_rule *);
 /* ---- introspection for measurement ----------------------------------------------------- */
 /* kernel classes for the per-kernel accounting below */
 enum b200_kernel { B200_K_LEV = 0, B200_K_COMPACT = 1, B200_K_PAIR_PROBE = 2, B200_K_SCATTER = 3, B200_K_EVAL_PATHS = 4, B200_K_EMIT = 5,
-                   B200_K_VEC_DIST = 6, B200_K_TOPK = 7, B200_K_VEC_GEMM = 8, B200_K_VEC_MERGE = 9, B200_K_SORT = 10, B200_K_COUNT = 11 };
+                   B200_K_VEC_DIST = 6, B200_K_TOPK = 7, B200_K_VEC_GEMM = 8, B200_K_VEC_MERGE = 9, B200_K_SORT = 10, B200_K_GEO = 11,
+                   B200_K_COUNT = 12 };
 typedef struct {
     uint64_t kernel_launches;     /* kernels launched by the library since the last reset */
     uint64_t device_steps;        /* host<->device round trips since the last reset */

@@ -22,7 +22,8 @@ MAX_SCORES = 12
 CRITERIA = {"words": 0, "typo": 1, "proximity": 2, "attribute": 3, "attributeRank": 4, "wordPosition": 5, "sort": 6, "exactness": 7}
 DEFAULT_CRITERIA = ["words", "typo", "proximity", "attributeRank", "sort", "wordPosition", "exactness"]  # criterion.rs:121-131
 TMS = {"last": 0, "all": 1, "frequency": 2}
-SCORE_KINDS = ["words", "typo", "proximity", "fid", "position", "exactAttribute", "exactWords", "vector", "skipped", "sort"]
+SCORE_KINDS = ["words", "typo", "proximity", "fid", "position", "exactAttribute", "exactWords", "vector", "skipped", "sort", "geo"]
+GEO_STRATEGIES = {"dynamic": 0, "iterative": 1, "rtree": 2}  # GeoSortStrategy::Dynamic / AlwaysIterative / AlwaysRtree
 DB_FACET_F64, DB_FACET_STRING = 10, 11
 NO_FIELD = 0xFFFF  # a sort field absent from the fields map
 ERRORS = {-1: "NO_DEVICE", -2: "CUDA", -3: "INVALID", -4: "UNSUPPORTED", -5: "CAPACITY", -6: "STATE"}
@@ -46,7 +47,9 @@ class _Batch(C.Structure):
                 ("offset", C.c_uint32), ("limit", C.c_uint32), ("words_limit", C.c_uint32), ("vectors", C.c_void_p),
                 ("mode", C.c_int32), ("semantic_ratio", C.c_float), ("universes", C.c_void_p), ("n_universe_words", C.c_uint64),
                 ("time_budget_ns", C.c_uint64), ("stop_after", C.c_int64), ("has_ranking_score_threshold", C.c_int32),
-                ("ranking_score_threshold", C.c_double), ("sort_begin", C.c_void_p), ("sort_fid", C.c_void_p), ("sort_asc", C.c_void_p)]
+                ("ranking_score_threshold", C.c_double), ("sort_begin", C.c_void_p), ("sort_fid", C.c_void_p), ("sort_asc", C.c_void_p),
+                ("sort_geo", C.c_void_p), ("sort_geo_point", C.c_void_p), ("geo_strategy", C.c_int32), ("geo_cache_size", C.c_uint32),
+                ("geo_max_bucket_size", C.c_uint64)]
 
 
 class _Results(C.Structure):
@@ -57,13 +60,13 @@ class _Results(C.Structure):
 
 class _Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("device_steps", C.c_uint64), ("posting_bytes", C.c_uint64), ("matrix_bytes", C.c_uint64),
-                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 11),
-                ("kernel_count", C.c_uint64 * 11), ("kernel_bytes", C.c_uint64 * 11), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
+                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 12),
+                ("kernel_count", C.c_uint64 * 12), ("kernel_bytes", C.c_uint64 * 12), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
                 ("hbm_bytes_staged", C.c_uint64), ("deferred", C.c_uint64), ("arena_peak_bytes", C.c_uint64),
                 ("eval_class_launches", C.c_uint64 * 9), ("eval_class_tiles", C.c_uint64 * 9)]
 
 
-KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort"]
+KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort", "geo"]
 
 
 def build_library(force=False):
@@ -96,6 +99,7 @@ def load_library():
         l.b200_stage_settings.argtypes = [C.c_void_p, C.POINTER(_Settings)]
         l.b200_stage_synonyms.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p)]
         l.b200_stage_finish.argtypes = [C.c_void_p]
+        l.b200_stage_geo_fields.argtypes = [C.c_void_p, C.c_uint16, C.c_uint16]
         l.b200_stage_embeddings.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p]
         l.b200_stage_embeddings_f16.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p]
         l.b200_stage_distribution.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float]
@@ -119,9 +123,17 @@ def load_library():
 
 
 SYMBOLS = ["b200_open", "b200_close", "b200_last_error", "b200_open_error", "b200_stage_dictionary", "b200_stage_db",
-           "b200_stage_documents_ids", "b200_stage_settings", "b200_stage_synonyms", "b200_stage_finish", "b200_stage_embeddings", "b200_stage_embeddings_f16", "b200_stage_distribution",
+           "b200_stage_documents_ids", "b200_stage_settings", "b200_stage_synonyms", "b200_stage_geo_fields", "b200_stage_finish", "b200_stage_embeddings", "b200_stage_embeddings_f16", "b200_stage_distribution",
            "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_graph_from_tokens",
            "b200_graph_free", "b200_rule_start", "b200_rule_next", "b200_rule_end", "b200_get_stats", "b200_reset_stats"]
+
+
+def parse_geo_point(name):
+    """(lat, lng) of a `_geoPoint(lat, lng)` sort entry's name, None for a field name (AscDesc parsing, asc_desc.rs)"""
+    import re
+
+    m = re.fullmatch(r"_geoPoint\(\s*([^,\s]+)\s*,\s*([^)\s]+)\s*\)", name)
+    return (float(m.group(1)), float(m.group(2))) if m else None
 
 
 def _p(a):
@@ -131,8 +143,9 @@ def _p(a):
 class SearchResult:
     """milli::SearchResult (search/mod.rs:526-535) for a batch of queries."""
 
-    def __init__(self, n, limit, sort_value=None):
+    def __init__(self, n, limit, sort_value=None, geo_point=None):
         self._sort_value = sort_value  # (fid, is_string, key index) -> (field name, value)
+        self._geo_point = geo_point  # docid -> its (lat, lng)
         self.sort_names = None  # per query: the field name of each sort rule, in rule order
         self.limit = max(limit, 1)
         L = self.limit
@@ -168,6 +181,9 @@ class SearchResult:
                     if self.sort_names is not None and s < len(self.sort_names[q]):
                         field = self.sort_names[q][s]  # the rule's field name (also for a field absent from the fields map)
                     row.append(("sort", field, bool(m & 2), value))
+                elif k == "geo":  # ScoreDetails::GeoSort: the bucket's first point, None for the Null bucket
+                    d = int(self.score_rank[q, i, s])
+                    row.append(("geo", bool(self.score_max[q, i, s] & 2), None if d == 0xFFFFFFFF else self._geo_point(d)))
                 else:
                     row.append((k, int(self.score_rank[q, i, s]), int(self.score_max[q, i, s])))
             out.append(row)
@@ -178,7 +194,7 @@ class Index:
     """The staged index: what milli reads from LMDB at query time, resident in HBM."""
 
     def __init__(self, image=None, *, device=0, criteria=None, authorize_typos=True, one_typo=5, two_typos=9, prefix_search=True,
-                 weights=None, exact_words=(), synonyms=None, facets=None):
+                 weights=None, exact_words=(), synonyms=None, facets=None, geo=None):
         self._l = load_library()
         h = C.c_void_p()
         rc = self._l.b200_open(device, C.byref(h))
@@ -188,18 +204,20 @@ class Index:
         self.dim = 0
         if image is not None:
             self.stage(image, criteria=criteria, authorize_typos=authorize_typos, one_typo=one_typo, two_typos=two_typos,
-                       prefix_search=prefix_search, weights=weights, exact_words=exact_words, synonyms=synonyms, facets=facets)
+                       prefix_search=prefix_search, weights=weights, exact_words=exact_words, synonyms=synonyms, facets=facets,
+                       geo=geo)
 
     def _ck(self, rc):
         if rc != 0:
             raise B200Error(rc, self._l.b200_last_error(self._h).decode())
 
     def stage(self, image, *, criteria=None, authorize_typos=True, one_typo=5, two_typos=9, prefix_search=True, weights=None, exact_words=(),
-              synonyms=None, facets=None):
+              synonyms=None, facets=None, geo=None):
         """image: anything with dict_bytes/dict_offsets/n_words, dbs[i].{key_bytes,key_offsets,val_bytes,val_offsets,n_keys},
         documents_ids_cbo, n_fields — i.e. the LMDB databases in their on-disk formats.  facets: a corpus.facets.FacetImage (or
         anything with `fields` (name -> fid) and built `f64_db` / `string_db`); criteria may name custom rules "asc:<field>" /
-        "desc:<field>" (Criterion::Asc / Desc)."""
+        "desc:<field>" (Criterion::Asc / Desc).  geo: the (lat fid, lng fid) of `_geo.lat` / `_geo.lng` for the GeoSort rule; by default
+        those of the facet image's `_geo.lat` / `_geo.lng` fields when it has them."""
         l = self._l
         self._facets = facets
         self._fields = dict(facets.fields) if facets is not None else {}
@@ -224,8 +242,21 @@ class Index:
             fr = (C.c_char_p * len(pairs))(*[k.encode() for k, _ in pairs])
             to = (C.c_char_p * len(pairs))(*[v.encode() for _, v in pairs])
             self._ck(l.b200_stage_synonyms(self._h, len(pairs), fr, to))
+        if geo is None and facets is not None and "_geo.lat" in facets.fields and "_geo.lng" in facets.fields:
+            geo = (facets.fields["_geo.lat"], facets.fields["_geo.lng"])
+        self._geo = geo
+        if geo is not None:
+            self._ck(l.b200_stage_geo_fields(self._h, geo[0], geo[1]))
         self._ck(l.b200_stage_finish(self._h))
         self.n_fields = image.n_fields
+
+    def geo_point(self, docid):
+        """the document's (lat, lng) as the GeoSort rule reads it (documents/geo_sort.rs:252-277): the smallest number value of each
+        coordinate field, else its smallest string value parsed as f64"""
+        if not hasattr(self, "_geo_points"):
+            from corpus.facets import geo_points
+            self._geo_points = geo_points(self._facets, *self._geo) if self._geo is not None else {}
+        return self._geo_points[docid]
 
     def _criterion(self, name):
         if name.startswith(("asc:", "desc:")):
@@ -242,7 +273,10 @@ class Index:
                 done = True
                 for item in sort_list:
                     f = item.rsplit(":", 1)[0]
-                    if f not in names:
+                    if parse_geo_point(f) is not None:  # every `_geoPoint` entry is a rule of its own
+                        names.append(f)
+                        kept.append(item)
+                    elif f not in names:
                         names.append(f)
                         kept.append(item)
             elif c.startswith(("asc:", "desc:")):
@@ -435,6 +469,7 @@ class Search:
         self._offset, self._limit, self._words_limit = 0, 20, 10
         self._universes, self._budget_ms, self._stop_after, self._threshold, self._want_candidates = None, None, None, None, False
         self._sort = None
+        self._geo_strategy, self._geo_max_bucket = (0, 1000), 1000
 
     def query(self, queries, stop_words=frozenset()):
         self._tokens = queries if isinstance(queries, TokenBatch) else TokenBatch([queries] if isinstance(queries, str) else list(queries), stop_words)
@@ -479,8 +514,19 @@ class Search:
         return self
 
     def sort(self, criteria):
-        """Search::sort_criteria: ["price:asc", "brand:desc", ...] for every query of the batch, or one such list per query"""
+        """Search::sort_criteria: ["price:asc", "_geoPoint(48.85, 2.35):desc", ...] for every query of the batch, or one such list
+        per query"""
         self._sort = criteria
+        return self
+
+    def geo_strategy(self, strategy, cache_size=1000):
+        """Search::geo_sort_strategy: "dynamic" (the default), "iterative" or "rtree", with its cache size"""
+        self._geo_strategy = (GEO_STRATEGIES[strategy], cache_size)
+        return self
+
+    def geo_max_bucket_size(self, n):
+        """Search::geo_max_bucket_size (default 1000)"""
+        self._geo_max_bucket = n
         return self
 
     def with_candidates(self):
@@ -494,7 +540,7 @@ class Search:
             n = self._vectors.shape[0] if self._vectors is not None else 1
             tokens = TokenBatch([""] * n)
         n = tokens.n_queries
-        res = SearchResult(n, self._limit, ix.sort_value)
+        res = SearchResult(n, self._limit, ix.sort_value, ix.geo_point)
         b = _Batch(n, _p(tokens.token_begin), _p(tokens.token_kind), _p(tokens.lemma_off), _p(tokens.lemma_bytes), TMS[self._tms],
                    1 if self._scoring == "detailed" else 0, self._offset, self._limit, self._words_limit,
                    _p(self._vectors) if self._vectors is not None else None, mode, ratio)
@@ -527,10 +573,16 @@ class Search:
             begin = np.zeros(n + 1, np.uint32)
             begin[1:] = np.cumsum([len(x) for x in per_q])
             items = [c.rsplit(":", 1) for x in per_q for c in x]
-            fid = np.asarray([ix.field_id(f) for f, _ in items] or [0], np.uint16)
+            geo = [parse_geo_point(f) for f, _ in items]
+            fid = np.asarray([NO_FIELD if g is not None else ix.field_id(f) for (f, _), g in zip(items, geo)] or [0], np.uint16)
             asc = np.asarray([1 if d == "asc" else 0 for _, d in items] or [0], np.uint8)
-            keep += [begin, fid, asc]
+            is_geo = np.asarray([g is not None for g in geo] or [0], np.uint8)
+            point = np.asarray([g if g is not None else (0.0, 0.0) for g in geo] or [(0.0, 0.0)], np.float64).reshape(-1)
+            keep += [begin, fid, asc, is_geo, point]
             b.sort_begin, b.sort_fid, b.sort_asc = _p(begin), _p(fid), _p(asc)
+            b.sort_geo, b.sort_geo_point = _p(is_geo), _p(point)
+        b.geo_strategy, b.geo_cache_size = self._geo_strategy
+        b.geo_max_bucket_size = self._geo_max_bucket
         b.time_budget_ns = 0 if self._budget_ms is None else max(1, int(self._budget_ms * 1e6))
         b.stop_after = -1 if self._stop_after is None else int(self._stop_after)
         b.has_ranking_score_threshold = int(self._threshold is not None)

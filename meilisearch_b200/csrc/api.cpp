@@ -160,6 +160,13 @@ int b200_stage_synonyms(b200_index *h, uint32_t n, const char *const *from_words
     for (uint32_t i = 0; i < n; i++) syn[split_ws(from_words[i])].push_back(split_ws(to_words[i]));
     return B200_OK;
 }
+int b200_stage_geo_fields(b200_index *h, uint16_t lat_fid, uint16_t lng_fid) {
+    std::lock_guard<std::mutex> g(h->e.mu);
+    if (h->e.staged) return h->e.fail(B200_ERR_STATE, "staging after b200_stage_finish: open a new handle");
+    h->e.hix.geo.lat_fid = lat_fid;
+    h->e.hix.geo.lng_fid = lng_fid;
+    return B200_OK;
+}
 int b200_stage_finish(b200_index *h) {
     return guarded(h, [&]() -> int {
         std::lock_guard<std::mutex> g(h->e.mu);

@@ -144,6 +144,9 @@ constexpr uint32_t SORT_MAX_LEVELS = 12;  // B200_MAX_SCORES
 constexpr uint32_t SORT_WINDOW = 2048;    // rows one CTA produces
 struct SortDesc {
     const unsigned long long *ub;          // dense universe bitmap, n_words words
+    const unsigned long long *exclude;     // nullptr, or documents left out of ub (n_words words)
+    const uint32_t *ids;                   // non-null: the universe is this docid list instead of ub
+    uint32_t n_ids;
     const uint32_t *keys[SORT_MAX_LEVELS]; // per level: u32[n_docs] sort keys, nullptr = every key 0 (a field without values)
     uint32_t bits[SORT_MAX_LEVELS + 1];    // significant bits of each tuple word ([n_levels]: the docid)
     uint32_t n_words, n_levels;
@@ -151,6 +154,43 @@ struct SortDesc {
     uint32_t *dst;                         // hi - lo docids
     uint32_t *dst_keys;                    // (hi - lo) x n_levels keys
     uint32_t *info;                        // out: universe passes, documents collected for the window
+};
+
+// one document of the GeoSort rule (geo.cu): lat_lng_to_xyz of its point (lib.rs:397-404, what the rtree holds), its point in
+// degrees and cos(lat) (the haversine's per-point factor), all computed on the host with the platform libm at staging
+struct GeoPoint {
+    double x, y, z, lat, lng, cos_lat;
+};
+// one window of the order of a GeoSort rule over (universe AND geo documents) (geo.cu), tuple (part, key_hi, key_lo, rdoc, docid):
+//   rtree order:     part 0, key = bits of the f64 squared chord distance to `q`, rdoc 0;
+//   iterative order: part 1 (0 when the whole order is iterative), key = floor(haversine metres) (ascending) or GEO_FLOOR_MAX minus
+//                    it (descending), rdoc = 0 (ascending) or GEO_DOC_MAX minus the docid (descending);
+//   mode 0: every document in rtree order; 1: every document in iterative order; 2: rtree order for the documents whose rtree tuple
+//   (key, docid) is at most `split`, iterative order after them (the Dynamic strategy's tail).
+constexpr uint32_t GEO_FLOOR_BITS = 25;  // floor(haversine) <= pi * 6371000 < 2^25
+constexpr uint32_t GEO_FLOOR_MAX = (1u << GEO_FLOOR_BITS) - 1;
+struct GeoDesc {
+    const unsigned long long *ub;   // universe, n_words words
+    const unsigned long long *geo;  // geo documents, n_words words
+    const GeoPoint *pts;            // per docid
+    double q[3];                    // rtree target: lat_lng_to_xyz(target), or of opposite_of(target) when descending
+    double t_lat, t_lng, t_cos_lat; // haversine target
+    unsigned long long split_key;   // mode 2
+    uint32_t split_doc;
+    uint32_t mode, asc, doc_max;
+    uint32_t n_words;
+    uint32_t bits[5];
+    uint32_t lo, hi;                // hi - lo <= SORT_WINDOW
+    uint32_t *dst;                  // hi - lo docids
+    double *dst_dist;               // their haversine distance to the target (metres)
+    unsigned long long *dst_key;    // their rtree key
+    uint32_t *info;                 // out: passes, documents collected
+};
+// geo_count_kernel: |universe AND geo| per query
+struct GeoCount {
+    const unsigned long long *ub, *geo;
+    uint32_t n_words;
+    uint32_t *out;
 };
 
 }  // namespace b200

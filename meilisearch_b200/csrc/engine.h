@@ -341,9 +341,17 @@ struct NcclId {
 struct GraphObj;  // S1: opaque query graph (engine_search.cpp)
 void free_graph(GraphObj *);
 
-struct SortRule {  // one sort ranking rule: a field and its direction
+struct SortRule {  // one sort ranking rule: a field and its direction, or a GeoSort rule (`_geoPoint(lat, lng)`) and its direction
     uint16_t fid;
     bool asc;
+    bool geo = false;
+    double lat = 0, lng = 0;
+};
+// GeoSortParameter of a search (documents/geo_sort.rs:12-63)
+struct GeoParams {
+    int strategy = 0;  // 0 Dynamic, 1 AlwaysIterative, 2 AlwaysRtree
+    uint32_t cache_size = 1000;
+    uint64_t max_bucket_size = 1000;
 };
 
 // The host side of a search is a few dozen threads working on the same per-query state.  On a two-socket host it is ~13 % faster
@@ -421,6 +429,14 @@ struct Engine {
     DevBuf<uint32_t> d_docids_out;  // n_queries x limit
     DevBuf<SortDesc> d_sort_desc;   // sort windows of a batch (sort.cu)
     DevBuf<uint32_t> d_sort_keys, d_sort_info;
+    // GeoSort (geo.cu): per docid its GeoPoint, the geo documents' bitmap; per batch the count / window descriptors and outputs
+    GeoPoint *d_geo_pts = nullptr;
+    unsigned long long *d_geo_ub = nullptr;
+    DevBuf<GeoCount> d_geo_count;
+    DevBuf<GeoDesc> d_geo_desc;
+    DevBuf<uint32_t> d_geo_u32;
+    DevBuf<double> d_geo_dist;
+    DevBuf<unsigned long long> d_geo_key;
     DevBuf<unsigned long long> d_universes;  // the batch's distinct filtered universes (documents_ids & filter), n_words64 words each
     DevBuf<uint32_t> d_rowtab;      // n_queries x n_words64: word -> (tag, row) of the query's current activation (ActDesc::row_tab)
     // lev buffers

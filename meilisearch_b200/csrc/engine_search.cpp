@@ -466,6 +466,14 @@ struct QState {
     bool sort_pending = false;
     uint32_t sort_lo = 0, sort_hi = 0;
     std::vector<uint32_t> sort_ids;  // the result window's docids
+    // a leading GeoSort rule (geo_windows): |universe AND geo| and the first rows of its order, with their haversine distance and
+    // rtree key; the Dynamic strategy's rtree / iterative split (the rtree tuple of rank geo_m - 1)
+    uint32_t geo_n = 0, geo_m = 0;
+    bool geo_split_known = false;
+    unsigned long long geo_split_key = 0;
+    uint32_t geo_split_doc = 0;
+    std::vector<uint32_t> geo_docs;
+    std::vector<double> geo_dist;
     // arena blocks of levels bucket_sort has left; the lane's driver returns them to its allocator at the start of its next step
     // (the emissions queued by the same advance() still read them: they run first on the lane's stream, before any new owner writes)
     std::vector<std::pair<size_t, size_t>> freed;
@@ -1670,7 +1678,7 @@ uint8_t score_kind_of(int rk) {
 double global_score_of(const std::vector<EScore> &sc) {
     uint64_t rk = 1, mx = 1;
     for (auto &x : sc) {
-        if (x.kind == B200_S_VECTOR || x.kind == B200_S_SORT) continue;  // no Rank (score_details.rs:110-154)
+        if (x.kind == B200_S_VECTOR || x.kind == B200_S_SORT || x.kind == B200_S_GEO_SORT) continue;  // no Rank (score_details.rs:110-154)
         rk = rk > 0 ? rk - 1 : 0;
         rk = rk * x.max_rank + x.rank;
         mx *= x.max_rank;
@@ -3131,125 +3139,378 @@ struct KeywordBatch {
             for (unsigned l = 0; l < n_lanes; l++) CU(cudaStreamSynchronize(lanes[l].stream), "sync candidates");
         return B200_OK;
     }
-    // ---- sort windows of the placeholder searches with sort rules (sort.cu), on the handle's stream
-    int sort_windows() {
-        std::vector<SortDesc> descs;
-        std::vector<std::pair<uint32_t, uint32_t>> owner;  // per window: query, first result row
-        size_t key_words = 0;
+    // ---- GeoSort as the first rule (geo.cu): the first rows of each query's geo order, as far as the result window needs them
+    // The order in which GeoSort's cache hands out the documents of G = universe AND geo is a tuple order (DESIGN.md §3): the
+    // first geo_m in rtree order, the rest in iterative order.  Its buckets are runs of that order (the chain of next_bucket,
+    // documents/geo_sort.rs:137-228), so the rows are produced from rank 0 up to the end of the bucket that holds the window's
+    // last rank: first up to that rank, then further while the chain goes on.
+    static constexpr double GEO_MARGIN_M = 1.0;  // GeoSortParameter::distance_error_margin
+    // the chain over rows [0, have): ends[k] = one past the last row of bucket k; a bucket is complete when a row breaks the chain
+    // after it, when it holds max_bucket_size rows, or when the rows are all of G
+    static void geo_chain(const QState &q, uint64_t cap, std::vector<uint32_t> &ends) {
+        const uint32_t have = (uint32_t)q.geo_docs.size();
+        ends.clear();
+        for (uint32_t s = 0; s < have;) {
+            const double d0 = q.geo_dist[s];
+            uint32_t e = s + 1;
+            while (e < have && e - s < cap && std::fabs(d0 - q.geo_dist[e]) <= GEO_MARGIN_M) e++;
+            ends.push_back(e);
+            s = e;
+        }
+    }
+    int geo_windows() {
+        const GeoParams gp{b->geo_strategy, b->geo_cache_size ? b->geo_cache_size : 1000u,
+                           b->geo_max_bucket_size ? b->geo_max_bucket_size : 1000ull};
+        std::vector<uint32_t> gq;
+        for (uint32_t i = 0; i < NQ; i++) {
+            const QState &q = *qs[i];
+            if (q.sort_pending && q.status == 0 && q.sort_rules[0].geo) gq.push_back(i);
+        }
+        if (gq.empty()) return B200_OK;
+        const uint32_t W = hix.n_words64;
+        // 1. n = |universe AND geo| per query
+        {
+            std::vector<GeoCount> cs(gq.size());
+            CU(eng.d_geo_count.reserve(gq.size()), "alloc geo counts");
+            CU(eng.d_geo_u32.reserve(gq.size()), "alloc geo counts");
+            for (size_t k = 0; k < gq.size(); k++) cs[k] = GeoCount{universe_of(*qs[gq[k]]), eng.d_geo_ub, W, eng.d_geo_u32.p + k};
+            CU(cudaMemcpyAsync(eng.d_geo_count.p, cs.data(), cs.size() * sizeof(GeoCount), cudaMemcpyHostToDevice, eng.stream), "H2D geo counts");
+            const size_t m0 = eng.mark();
+            CU(launch_geo_count(eng.stream, eng.d_geo_count.p, (uint32_t)gq.size()), "geo_count");
+            eng.time_kernel(B200_K_GEO, m0, eng.mark(), 0);
+            std::vector<uint32_t> n(gq.size());
+            CU(cudaMemcpyAsync(n.data(), eng.d_geo_u32.p, n.size() * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H geo counts");
+            CU(cudaStreamSynchronize(eng.stream), "sync geo counts");
+            stats.h2d_bytes += cs.size() * sizeof(GeoCount);
+            stats.d2h_bytes += n.size() * 4;
+            stats.kernel_bytes[B200_K_GEO] += (uint64_t)gq.size() * W * 16;
+            for (size_t k = 0; k < gq.size(); k++) {
+                QState &q = *qs[gq[k]];
+                q.geo_n = n[k];
+                // documents in rtree order (documents/geo_sort.rs:48-63,80-118): Dynamic(c) fills the cache from the rtree while at
+                // least c candidates remain, c at a time, and sorts the rest iteratively in one fill
+                q.geo_m = gp.strategy == 2 ? q.geo_n : gp.strategy == 1 ? 0u : (q.geo_n >= gp.cache_size ? q.geo_n - q.geo_n % gp.cache_size : 0u);
+            }
+        }
+        // 2. rows of the order, in rounds, until every query's window ends in a complete bucket
         const uint32_t doc_bits = hix.n_docs > 1 ? 32u - (uint32_t)__builtin_clz(hix.n_docs - 1) : 0u;
-        // A query's ranks [sort_lo, sort_hi) are produced with one more rank on each side where the universe has it: under Skip a
-        // bucket of at most one document is returned with the scores of the rules above it only (bucket_sort.rs:299-312), and
-        // whether a document's group of equal keys is a singleton shows in its neighbours.
-        std::vector<uint32_t> q_first(NQ, 0), q_elo(NQ, 0);
-        size_t id_words = 0;
+        std::vector<uint32_t> want(NQ, 0), need(NQ, 0);  // rows asked for; rows the window itself covers
+        std::vector<uint32_t> active;
+        for (uint32_t i : gq) {
+            QState &q = *qs[i];
+            const uint32_t ehi = (uint32_t)std::min<uint64_t>(q.univ_count, (uint64_t)q.sort_hi + 1), elo = q.sort_lo > 0 ? q.sort_lo - 1 : 0;
+            if (elo < q.geo_n) {
+                want[i] = need[i] = std::min(q.geo_n, ehi);
+                active.push_back(i);
+            }
+        }
+        while (!active.empty()) {
+            std::vector<GeoDesc> descs;
+            std::vector<std::pair<uint32_t, bool>> owner;  // query, split select
+            size_t rows = 0;
+            for (uint32_t i : active) {
+                QState &q = *qs[i];
+                const SortRule &rule = q.sort_rules[0];
+                const bool need_split = q.geo_m > 0 && q.geo_m < q.geo_n && want[i] > q.geo_m && !q.geo_split_known;
+                GeoDesc d{};
+                d.ub = universe_of(q);
+                d.geo = eng.d_geo_ub;
+                d.pts = eng.d_geo_pts;
+                d.n_words = W;
+                // rtree target: lat_lng_to_xyz of the point, or of opposite_of(point) when descending (documents/geo_sort.rs:96-118,280-290)
+                double la = rule.lat, ln = rule.lng;
+                if (!rule.asc) {
+                    la = -la;
+                    ln = ln > 0. ? ln - 180. : ln + 180.;
+                }
+                const double to_rad = M_PI / 180.0, rla = la * to_rad, rln = ln * to_rad;
+                d.q[0] = std::cos(rla) * std::cos(rln);
+                d.q[1] = std::cos(rla) * std::sin(rln);
+                d.q[2] = std::sin(rla);
+                d.t_lat = rule.lat;
+                d.t_lng = rule.lng;
+                d.t_cos_lat = std::cos(rule.lat * to_rad);
+                d.asc = rule.asc ? 1 : 0;
+                d.doc_max = doc_bits ? (uint32_t)((1ull << doc_bits) - 1) : 0u;
+                const uint32_t have = (uint32_t)q.geo_docs.size();
+                uint32_t lo = have, hi = want[i];
+                if (need_split) {
+                    d.mode = 0;
+                    lo = q.geo_m - 1;
+                    hi = q.geo_m;
+                } else if (q.geo_m == q.geo_n || want[i] <= q.geo_m)
+                    d.mode = 0;
+                else if (q.geo_m == 0)
+                    d.mode = 1;
+                else {
+                    d.mode = 2;
+                    d.split_key = q.geo_split_key;
+                    d.split_doc = q.geo_split_doc;
+                }
+                const bool iter_desc = d.mode != 0 && !rule.asc;
+                const uint32_t bits[5] = {d.mode == 2 ? 1u : 0u, d.mode == 1 ? 0u : 32u, d.mode == 1 ? GEO_FLOOR_BITS : 32u, iter_desc ? doc_bits : 0u, doc_bits};
+                for (int w = 0; w < 5; w++) d.bits[w] = bits[w];
+                for (uint32_t at = lo; at < hi; at += SORT_WINDOW) {
+                    d.lo = at;
+                    d.hi = std::min<uint32_t>(hi, at + SORT_WINDOW);
+                    d.dst = reinterpret_cast<uint32_t *>((uintptr_t)rows);  // row offsets, made pointers below
+                    rows += d.hi - d.lo;
+                    descs.push_back(d);
+                    owner.emplace_back(i, need_split);
+                }
+            }
+            const size_t n = descs.size();
+            CU(eng.d_geo_desc.reserve(n), "alloc geo windows");
+            CU(eng.d_geo_u32.reserve(rows + 2 * n), "alloc geo rows");
+            CU(eng.d_geo_dist.reserve(rows), "alloc geo rows");
+            CU(eng.d_geo_key.reserve(rows), "alloc geo rows");
+            for (size_t k = 0; k < n; k++) {
+                const size_t off = (uintptr_t)descs[k].dst;
+                descs[k].dst = eng.d_geo_u32.p + off;
+                descs[k].dst_dist = eng.d_geo_dist.p + off;
+                descs[k].dst_key = eng.d_geo_key.p + off;
+                descs[k].info = eng.d_geo_u32.p + rows + 2 * k;
+            }
+            CU(cudaMemcpyAsync(eng.d_geo_desc.p, descs.data(), n * sizeof(GeoDesc), cudaMemcpyHostToDevice, eng.stream), "H2D geo windows");
+            const size_t m0 = eng.mark();
+            CU(launch_geo_window(eng.stream, eng.d_geo_desc.p, (uint32_t)n), "geo_window");
+            eng.time_kernel(B200_K_GEO, m0, eng.mark(), 0);
+            std::vector<uint32_t> u32(rows + 2 * n);
+            std::vector<double> dist(rows);
+            std::vector<unsigned long long> key(rows);
+            CU(cudaMemcpyAsync(u32.data(), eng.d_geo_u32.p, u32.size() * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H geo rows");
+            CU(cudaMemcpyAsync(dist.data(), eng.d_geo_dist.p, rows * 8, cudaMemcpyDeviceToHost, eng.stream), "D2H geo rows");
+            CU(cudaMemcpyAsync(key.data(), eng.d_geo_key.p, rows * 8, cudaMemcpyDeviceToHost, eng.stream), "D2H geo rows");
+            CU(cudaStreamSynchronize(eng.stream), "sync geo rows");
+            eng.resolve_timers();
+            stats.h2d_bytes += n * sizeof(GeoDesc);
+            stats.d2h_bytes += u32.size() * 4 + rows * 16;
+            for (size_t k = 0; k < n; k++) {
+                QState &q = *qs[owner[k].first];
+                const GeoDesc &d = descs[k];
+                const size_t off = d.dst - eng.d_geo_u32.p, nr = d.hi - d.lo;
+                // algorithmic bytes: every pass reads the two bitmaps and a GeoPoint per document of G; the rows are written out
+                stats.kernel_bytes[B200_K_GEO] += (uint64_t)u32[rows + 2 * k] * (W * 16ull + q.geo_n * (uint64_t)sizeof(GeoPoint)) + nr * 20ull;
+                if (u32[rows + 2 * k + 1] != nr) {
+                    q.status = B200_ERR_CUDA;
+                    q.error = "internal: geo window collected a different number of documents than its rank range";
+                    continue;
+                }
+                if (owner[k].second) {
+                    q.geo_split_known = true;
+                    q.geo_split_key = key[off];
+                    q.geo_split_doc = u32[off];
+                    continue;
+                }
+                q.geo_docs.insert(q.geo_docs.end(), u32.begin() + off, u32.begin() + off + nr);
+                q.geo_dist.insert(q.geo_dist.end(), dist.begin() + off, dist.begin() + off + nr);
+            }
+            std::vector<uint32_t> next, ends;
+            for (uint32_t i : active) {
+                QState &q = *qs[i];
+                if (q.status != 0) continue;
+                const uint32_t have = (uint32_t)q.geo_docs.size();
+                if (have < want[i]) {  // waited for its split
+                    next.push_back(i);
+                    continue;
+                }
+                geo_chain(q, gp.max_bucket_size, ends);
+                const size_t k = std::upper_bound(ends.begin(), ends.end(), need[i] - 1) - ends.begin();  // the bucket of the last rank
+                const uint32_t e = ends[k], s = k ? ends[k - 1] : 0;
+                if (e < have || e - s == gp.max_bucket_size || have == q.geo_n) continue;  // that bucket is complete
+                want[i] = std::min<uint32_t>(q.geo_n, have + std::max<uint32_t>(have, 256));
+                next.push_back(i);
+            }
+            active.swap(next);
+        }
+        return B200_OK;
+    }
+    // ---- sort windows of the placeholder searches with sort rules (sort.cu), on the handle's stream
+    // A query's ranks [sort_lo, sort_hi) are produced with one more rank on each side where the universe has it: under Skip a bucket
+    // of at most one document is returned with the scores of the rules above it only (bucket_sort.rs:299-312), and whether a
+    // document's group of equal keys is a singleton shows in its neighbours.  Without a GeoSort rule those ranks are one segment of
+    // the universe's (keys, docid) order.  With a leading GeoSort rule (geo_windows) they are cut into segments along its buckets:
+    // each geo bucket is ordered by the following rules' (keys, docid) over its docid list, and the ranks past the geo documents by
+    // the same over the universe without them (the Null bucket); the GeoSort rule's key is the bucket's index.
+    int sort_windows() {
+        struct Seg {
+            uint32_t q, ext_row;    // query, first extended-window row
+            uint32_t first_level;   // 1: level 0 is a GeoSort rule whose key is `bucket`
+            uint32_t bucket;
+        };
+        std::vector<SortDesc> descs;
+        std::vector<Seg> owner;  // per window
+        std::vector<uint32_t> lists;  // docids of the geo buckets the windows read, uploaded with the windows
+        std::vector<std::pair<size_t, size_t>> list_of;  // per window: (offset into lists, length), length 0 = none
+        size_t key_words = 0, id_words = 0;
+        const uint32_t doc_bits = hix.n_docs > 1 ? 32u - (uint32_t)__builtin_clz(hix.n_docs - 1) : 0u;
+        std::vector<uint32_t> q_elo(NQ, 0);
+        std::vector<std::vector<uint32_t>> geo_p0(NQ);  // per query: the first docid of each geo bucket
+        auto add_windows = [&](QState &q, const SortDesc &proto, uint32_t lo, uint32_t hi, Seg seg, size_t list_off, size_t list_len) {
+            const uint32_t Lf = (uint32_t)q.sort_rules.size() - seg.first_level;
+            for (uint32_t at = lo; at < hi; at += SORT_WINDOW) {
+                SortDesc d = proto;
+                d.lo = at;
+                d.hi = std::min<uint32_t>(hi, at + SORT_WINDOW);
+                d.dst = reinterpret_cast<uint32_t *>((uintptr_t)id_words);  // offsets, made pointers below
+                id_words += d.hi - d.lo;
+                d.dst_keys = reinterpret_cast<uint32_t *>((uintptr_t)key_words);
+                key_words += (size_t)(d.hi - d.lo) * Lf;
+                descs.push_back(d);
+                Seg s = seg;
+                s.ext_row += at - lo;
+                owner.push_back(s);
+                list_of.emplace_back(list_off, list_len);
+            }
+        };
         for (uint32_t i = 0; i < NQ; i++) {
             QState &q = *qs[i];
             if (!q.sort_pending || q.status != 0) continue;
-            const uint32_t L = (uint32_t)q.sort_rules.size();
+            const uint32_t L = (uint32_t)q.sort_rules.size(), first = q.sort_rules[0].geo ? 1u : 0u;
             const uint32_t elo = q.sort_lo > 0 ? q.sort_lo - 1 : 0, ehi = (uint32_t)std::min<uint64_t>(q.univ_count, (uint64_t)q.sort_hi + 1);
-            q_first[i] = (uint32_t)descs.size();
             q_elo[i] = elo;
-            for (uint32_t lo = elo; lo < ehi; lo += SORT_WINDOW) {
-                SortDesc d{};
-                d.ub = universe_of(q);
-                d.n_words = hix.n_words64;
-                d.n_levels = L;
-                for (uint32_t l = 0; l < L; l++) {
-                    auto it = hix.sort_fields.find(q.sort_rules[l].fid);
-                    if (it == hix.sort_fields.end()) continue;  // no value anywhere: one Null bucket
-                    const uint32_t V = it->second.n_values();
-                    d.keys[l] = it->second.d_key[q.sort_rules[l].asc ? 0 : 1];
-                    d.bits[l] = V ? 32u - (uint32_t)__builtin_clz(V) : 0u;
+            SortDesc proto{};
+            proto.ub = universe_of(q);
+            proto.n_words = hix.n_words64;
+            proto.n_levels = L - first;
+            for (uint32_t l = first; l < L; l++) {
+                auto it = hix.sort_fields.find(q.sort_rules[l].fid);
+                if (it == hix.sort_fields.end()) continue;  // no value anywhere: one Null bucket
+                const uint32_t V = it->second.n_values();
+                proto.keys[l - first] = it->second.d_key[q.sort_rules[l].asc ? 0 : 1];
+                proto.bits[l - first] = V ? 32u - (uint32_t)__builtin_clz(V) : 0u;
+            }
+            proto.bits[L - first] = doc_bits;
+            if (!first) {
+                add_windows(q, proto, elo, ehi, Seg{i, 0, 0, 0}, 0, 0);
+                continue;
+            }
+            // geo buckets over the rows geo_windows produced, then the Null bucket
+            const uint64_t cap = b->geo_max_bucket_size ? b->geo_max_bucket_size : 1000ull;
+            std::vector<uint32_t> ends;
+            if (elo < q.geo_n) geo_chain(q, cap, ends);
+            for (uint32_t bucket = 0, bs = 0; bucket < ends.size() && bs < ehi; bs = ends[bucket++]) {
+                const uint32_t be = ends[bucket];
+                geo_p0[i].push_back(q.geo_docs[bs]);
+                if (be > elo) {
+                    SortDesc d = proto;
+                    d.n_ids = be - bs;  // d.ids: set below from list_of
+                    const size_t off = lists.size();
+                    lists.insert(lists.end(), q.geo_docs.begin() + bs, q.geo_docs.begin() + be);
+                    const uint32_t lo = std::max(elo, bs), hi = std::min(ehi, be);
+                    add_windows(q, d, lo - bs, hi - bs, Seg{i, lo - elo, 1, bucket}, off, be - bs);
                 }
-                d.bits[L] = doc_bits;
-                d.lo = lo;
-                d.hi = std::min<uint32_t>(ehi, lo + SORT_WINDOW);
-                d.dst = reinterpret_cast<uint32_t *>((uintptr_t)id_words);  // offsets, made pointers below
-                id_words += d.hi - d.lo;
-                d.dst_keys = reinterpret_cast<uint32_t *>((uintptr_t)key_words);  // offset, made a pointer below
-                key_words += (size_t)(d.hi - d.lo) * L;
-                descs.push_back(d);
-                owner.emplace_back(i, lo - elo);
+            }
+            if (ehi > q.geo_n) {
+                SortDesc d = proto;
+                d.exclude = eng.d_geo_ub;
+                const uint32_t lo = std::max(elo, q.geo_n);
+                add_windows(q, d, lo - q.geo_n, ehi - q.geo_n, Seg{i, lo - elo, 1, 0xffffffffu}, 0, 0);
             }
         }
-        if (!descs.empty()) {
-            const size_t n = descs.size();
-            CU(eng.d_sort_keys.reserve(std::max<size_t>(1, key_words + id_words)), "alloc sort keys");
-            CU(eng.d_sort_info.reserve(2 * n), "alloc sort info");
-            CU(eng.d_sort_desc.reserve(n), "alloc sort windows");
-            for (size_t k = 0; k < n; k++) {
-                descs[k].dst_keys = eng.d_sort_keys.p + (uintptr_t)descs[k].dst_keys;
-                descs[k].dst = eng.d_sort_keys.p + key_words + (uintptr_t)descs[k].dst;
-                descs[k].info = eng.d_sort_info.p + 2 * k;
+        if (descs.empty()) return B200_OK;
+        const size_t n = descs.size();
+        CU(eng.d_sort_keys.reserve(std::max<size_t>(1, key_words + id_words + lists.size())), "alloc sort keys");
+        CU(eng.d_sort_info.reserve(2 * n), "alloc sort info");
+        CU(eng.d_sort_desc.reserve(n), "alloc sort windows");
+        uint32_t *d_lists = eng.d_sort_keys.p + key_words + id_words;
+        for (size_t k = 0; k < n; k++) {
+            descs[k].dst_keys = eng.d_sort_keys.p + (uintptr_t)descs[k].dst_keys;
+            descs[k].dst = eng.d_sort_keys.p + key_words + (uintptr_t)descs[k].dst;
+            descs[k].info = eng.d_sort_info.p + 2 * k;
+            if (list_of[k].second) descs[k].ids = d_lists + list_of[k].first;
+        }
+        if (!lists.empty())
+            CU(cudaMemcpyAsync(d_lists, lists.data(), lists.size() * 4, cudaMemcpyHostToDevice, eng.stream), "H2D geo buckets");
+        CU(cudaMemcpyAsync(eng.d_sort_desc.p, descs.data(), n * sizeof(SortDesc), cudaMemcpyHostToDevice, eng.stream), "H2D sort windows");
+        const size_t m0 = eng.mark();
+        CU(launch_sort_window(eng.stream, eng.d_sort_desc.p, (uint32_t)n), "sort_window");
+        eng.time_kernel(B200_K_SORT, m0, eng.mark(), 0);
+        std::vector<uint32_t> keys(key_words + id_words), info(2 * n);
+        CU(cudaMemcpyAsync(keys.data(), eng.d_sort_keys.p, (key_words + id_words) * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H sort keys");
+        CU(cudaMemcpyAsync(info.data(), eng.d_sort_info.p, 2 * n * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H sort info");
+        CU(cudaStreamSynchronize(eng.stream), "sync sort");
+        eng.resolve_timers();
+        stats.h2d_bytes += n * sizeof(SortDesc) + lists.size() * 4;
+        stats.d2h_bytes += (key_words + id_words) * 4 + 2 * n * 4;
+        // the extended windows: per query its rows' docids and all L keys
+        std::vector<std::vector<uint32_t>> ext_ids(NQ), ext_keys(NQ);
+        for (uint32_t i = 0; i < NQ; i++) {
+            QState &q = *qs[i];
+            if (!q.sort_pending || q.status != 0) continue;
+            const uint32_t n_ext = (uint32_t)std::min<uint64_t>(q.univ_count, (uint64_t)q.sort_hi + 1) - q_elo[i];
+            ext_ids[i].assign(n_ext, 0);
+            ext_keys[i].assign((size_t)n_ext * q.sort_rules.size(), 0);
+        }
+        for (size_t k = 0; k < n; k++) {
+            const SortDesc &d = descs[k];
+            const Seg &sg = owner[k];
+            QState &q = *qs[sg.q];
+            const uint32_t rows = d.hi - d.lo, Lf = d.n_levels, L = (uint32_t)q.sort_rules.size();
+            // algorithmic bytes: every pass reads the universe (words, or a list) and one key per document; the window writes docids + keys
+            const uint64_t set_bytes = d.ids ? d.n_ids * 4ull : hix.n_words64 * 8ull * (d.exclude ? 2 : 1);
+            stats.kernel_bytes[B200_K_SORT] += (uint64_t)info[2 * k] * (set_bytes + (d.ids ? d.n_ids : q.univ_count) * 4ull) + (uint64_t)rows * 4 * (Lf + 1);
+            if (info[2 * k + 1] != rows) {
+                q.status = B200_ERR_CUDA;
+                q.error = "internal: sort window collected a different number of documents than its rank range";
+                continue;
             }
-            CU(cudaMemcpyAsync(eng.d_sort_desc.p, descs.data(), n * sizeof(SortDesc), cudaMemcpyHostToDevice, eng.stream), "H2D sort windows");
-            const size_t m0 = eng.mark();
-            CU(launch_sort_window(eng.stream, eng.d_sort_desc.p, (uint32_t)n), "sort_window");
-            eng.time_kernel(B200_K_SORT, m0, eng.mark(), 0);
-            std::vector<uint32_t> keys(key_words + id_words), info(2 * n);
-            CU(cudaMemcpyAsync(keys.data(), eng.d_sort_keys.p, (key_words + id_words) * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H sort keys");
-            CU(cudaMemcpyAsync(info.data(), eng.d_sort_info.p, 2 * n * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H sort info");
-            CU(cudaStreamSynchronize(eng.stream), "sync sort");
-            eng.resolve_timers();
-            stats.h2d_bytes += n * sizeof(SortDesc);
-            stats.d2h_bytes += (key_words + id_words) * 4 + 2 * n * 4;
-            for (size_t k = 0; k < n; k++) {
-                const SortDesc &d = descs[k];
-                QState &q = *qs[owner[k].first];
-                const uint32_t rows = d.hi - d.lo, L = d.n_levels;
-                // algorithmic bytes: every pass reads the universe words and one key per document; the window writes docids + keys
-                stats.kernel_bytes[B200_K_SORT] += (uint64_t)info[2 * k] * (hix.n_words64 * 8ull + q.univ_count * 4ull) + (uint64_t)rows * 4 * (L + 1);
-                if (info[2 * k + 1] != rows) {
-                    q.status = B200_ERR_CUDA;
-                    q.error = "internal: sort window collected a different number of documents than its rank range";
-                }
+            const uint32_t *ids = keys.data() + key_words + (d.dst - (eng.d_sort_keys.p + key_words));
+            const uint32_t *kp = keys.data() + (d.dst_keys - eng.d_sort_keys.p);
+            for (uint32_t r = 0; r < rows; r++) {
+                const size_t e = sg.ext_row + r;
+                ext_ids[sg.q][e] = ids[r];
+                if (sg.first_level) ext_keys[sg.q][e * L] = sg.bucket;
+                for (uint32_t l = 0; l < Lf; l++) ext_keys[sg.q][e * L + sg.first_level + l] = kp[(size_t)r * Lf + l];
             }
-            for (uint32_t i = 0; i < NQ; i++) {
-                QState &q = *qs[i];
-                if (!q.sort_pending || q.status != 0) continue;
-                const SortDesc &d0 = descs[q_first[i]];
-                const uint32_t L = d0.n_levels, elo = q_elo[i];
-                const uint32_t n_ext = (uint32_t)std::min<uint64_t>(q.univ_count, (uint64_t)q.sort_hi + 1) - elo;
-                const uint32_t *ids = keys.data() + key_words + ((uintptr_t)d0.dst - (uintptr_t)(eng.d_sort_keys.p + key_words)) / 4;
-                const uint32_t *kp = keys.data() + ((uintptr_t)d0.dst_keys - (uintptr_t)eng.d_sort_keys.p) / 4;
-                auto shares = [&](uint32_t a, uint32_t b, uint32_t n_keys) {  // keys [0, n_keys) of ext rows a and b agree
-                    for (uint32_t l = 0; l < n_keys; l++)
-                        if (kp[(size_t)a * L + l] != kp[(size_t)b * L + l]) return false;
-                    return true;
-                };
-                q.sort_ids.assign(ids + (q.sort_lo - elo), ids + (q.sort_hi - elo));
-                for (uint32_t j = 0; j < q.sort_hi - q.sort_lo; j++) {
-                    const uint32_t e = q.sort_lo - elo + j;
-                    // Under Skip a document leaves bucket_sort early at the first rule l (top down) where either
-                    //  - the rule's remaining universe is that document alone (bucket_sort.rs:196-204): it is the last of its group of
-                    //    equal keys [0, l) and no other document of that group shares its key l -> the scores of the rules above l;
-                    //  - the rule's bucket holding it has no other document (:299-312) -> the scores of rules [0, l].
-                    uint32_t n_sc = L;
-                    if (skip_scoring)
-                        for (uint32_t l = 0; l < L; l++) {
-                            const bool has_prev = e > 0, has_next = e + 1 < n_ext;
-                            const bool last_of_group = !(has_next && shares(e, e + 1, l));
-                            const bool alone = !(has_prev && shares(e, e - 1, l + 1)) && !(has_next && shares(e, e + 1, l + 1));
-                            if (last_of_group && alone) {
-                                n_sc = l;
-                                break;
-                            }
-                            if (alone) {
-                                n_sc = l + 1;
-                                break;
-                            }
+        }
+        for (uint32_t i = 0; i < NQ; i++) {
+            QState &q = *qs[i];
+            if (!q.sort_pending || q.status != 0) continue;
+            const uint32_t L = (uint32_t)q.sort_rules.size(), elo = q_elo[i];
+            const uint32_t n_ext = (uint32_t)ext_ids[i].size();
+            const uint32_t *kp = ext_keys[i].data();
+            auto shares = [&](uint32_t a, uint32_t b, uint32_t n_keys) {  // keys [0, n_keys) of ext rows a and b agree
+                for (uint32_t l = 0; l < n_keys; l++)
+                    if (kp[(size_t)a * L + l] != kp[(size_t)b * L + l]) return false;
+                return true;
+            };
+            q.sort_ids.assign(ext_ids[i].begin() + (q.sort_lo - elo), ext_ids[i].begin() + (q.sort_hi - elo));
+            for (uint32_t j = 0; j < q.sort_hi - q.sort_lo; j++) {
+                const uint32_t e = q.sort_lo - elo + j;
+                // Under Skip a document leaves bucket_sort early at the first rule l (top down) where either
+                //  - the rule's remaining universe is that document alone (bucket_sort.rs:196-204): it is the last of its group of
+                //    equal keys [0, l) and no other document of that group shares its key l -> the scores of the rules above l;
+                //  - the rule's bucket holding it has no other document (:299-312) -> the scores of rules [0, l].
+                uint32_t n_sc = L;
+                if (skip_scoring)
+                    for (uint32_t l = 0; l < L; l++) {
+                        const bool has_prev = e > 0, has_next = e + 1 < n_ext;
+                        const bool last_of_group = !(has_next && shares(e, e + 1, l));
+                        const bool alone = !(has_prev && shares(e, e - 1, l + 1)) && !(has_next && shares(e, e + 1, l + 1));
+                        if (last_of_group && alone) {
+                            n_sc = l;
+                            break;
                         }
-                    std::vector<EScore> &sc = q.scores[j];
-                    sc.clear();
-                    for (uint32_t l = 0; l < n_sc; l++) {
-                        const SortRule &rule = q.sort_rules[l];
-                        const uint32_t key = kp[(size_t)e * L + l];
-                        auto it = hix.sort_fields.find(rule.fid);
-                        bool is_string = false;
-                        uint32_t key_index = 0xffffffffu;
-                        if (it != hix.sort_fields.end() && key < it->second.n_values()) it->second.decode(rule.asc, key, is_string, key_index);
-                        sc.push_back(EScore{B200_S_SORT, key_index, (uint32_t)rule.fid << 2 | (rule.asc ? 2u : 0u) | (is_string ? 1u : 0u), -1.f});
+                        if (alone) {
+                            n_sc = l + 1;
+                            break;
+                        }
                     }
+                std::vector<EScore> &sc = q.scores[j];
+                sc.clear();
+                for (uint32_t l = 0; l < n_sc; l++) {
+                    const SortRule &rule = q.sort_rules[l];
+                    const uint32_t key = kp[(size_t)e * L + l];
+                    if (rule.geo) {  // ScoreDetails::GeoSort: the bucket's first point, None for the Null bucket
+                        sc.push_back(EScore{B200_S_GEO_SORT, key == 0xffffffffu ? key : geo_p0[i][key], rule.asc ? 2u : 0u, -1.f});
+                        continue;
+                    }
+                    auto it = hix.sort_fields.find(rule.fid);
+                    bool is_string = false;
+                    uint32_t key_index = 0xffffffffu;
+                    if (it != hix.sort_fields.end() && key < it->second.n_values()) it->second.decode(rule.asc, key, is_string, key_index);
+                    sc.push_back(EScore{B200_S_SORT, key_index, (uint32_t)rule.fid << 2 | (rule.asc ? 2u : 0u) | (is_string ? 1u : 0u), -1.f});
                 }
             }
         }
@@ -3334,6 +3595,7 @@ struct KeywordBatch {
     // after the step loop: statistics, sort windows, results and reports; the per-query state is freed in the background
     int finish_batch() {
         int rc = fold_lane_stats();
+        if (rc == B200_OK) rc = geo_windows();
         if (rc == B200_OK) rc = sort_windows();
         if (rc != B200_OK) return rc;
         const auto t_out = clk::now();
@@ -3349,7 +3611,8 @@ struct KeywordBatch {
 }  // namespace
 
 // The sort rules of query qi (search/new/mod.rs:351-416, 651-716): the `Sort` criterion expands to the query's `sort` list at its
-// position, once; Asc(f) / Desc(f) criteria add one rule each; a field sorted earlier in the list is skipped.  Sort is built for
+// position, once; Asc(f) / Desc(f) criteria add one rule each; a field sorted earlier in the list is skipped; every `_geoPoint`
+// entry adds a GeoSort rule.  Sort is built for
 // placeholder keyword searches; every other search with sort rules is refused with B200_ERR_UNSUPPORTED rather than answered without
 // them.  Returns B200_OK with the rules in `out`, or the code the query fails with and `why`.
 int Engine::sort_rules(const b200_query_batch *b, uint32_t qi, bool semantic, bool placeholder, std::vector<SortRule> &out, const char *&why) const {
@@ -3372,6 +3635,16 @@ int Engine::sort_rules(const b200_query_batch *b, uint32_t qi, bool semantic, bo
         why = "sort_begin without sort_fid / sort_asc";
         return B200_ERR_INVALID;
     }
+    bool has_geo = false;
+    for (uint32_t k = s0; k < s1 && b->sort_geo; k++) has_geo |= b->sort_geo[k] != 0;
+    if (has_geo && !b->sort_geo_point) {
+        why = "sort_geo without sort_geo_point";
+        return B200_ERR_INVALID;
+    }
+    if (has_geo && (b->geo_strategy < 0 || b->geo_strategy > 2)) {
+        why = "geo_strategy is not 0 (Dynamic), 1 (AlwaysIterative) or 2 (AlwaysRtree)";
+        return B200_ERR_INVALID;
+    }
     std::vector<SortRule> sr;
     std::vector<uint16_t> sorted;
     bool sort_done = false;
@@ -3385,7 +3658,12 @@ int Engine::sort_rules(const b200_query_batch *b, uint32_t qi, bool semantic, bo
     for (int c : hix.settings.criteria) {
         if (c == B200_C_SORT && !sort_done) {
             sort_done = true;
-            for (uint32_t k = s0; k < s1; k++) add(b->sort_fid[k], b->sort_asc[k] != 0);
+            for (uint32_t k = s0; k < s1; k++) {
+                if (b->sort_geo && b->sort_geo[k])  // one GeoSort rule per entry, never deduplicated (geo_sorted is never set)
+                    sr.push_back(SortRule{0xFFFF, b->sort_asc[k] != 0, true, b->sort_geo_point[2 * k], b->sort_geo_point[2 * k + 1]});
+                else
+                    add(b->sort_fid[k], b->sort_asc[k] != 0);
+            }
         } else if (c & 0x10000)
             add((uint16_t)(c & 0xffff), true);
         else if (c & 0x20000)
@@ -3400,6 +3678,8 @@ int Engine::sort_rules(const b200_query_batch *b, uint32_t qi, bool semantic, bo
         why = "more than B200_MAX_SCORES sort rules";
     else if (b->stop_after >= 0)
         why = "stop_after together with a sort rule (the sort window is one device step; its polls are not counted)";
+    else if (std::any_of(sr.begin() + 1, sr.end(), [](const SortRule &x) { return x.geo; }))
+        why = "GeoSort rule after the first rule of the stack (it is built as the first rule only)";
     else {
         out = std::move(sr);
         return B200_OK;

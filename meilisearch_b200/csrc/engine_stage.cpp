@@ -91,6 +91,13 @@ Engine::~Engine() {
     for (auto &kv : hix.sort_fields)
         for (auto p : kv.second.d_key)
             if (p) cudaFree(p);
+    if (d_geo_pts) cudaFree(d_geo_pts);
+    if (d_geo_ub) cudaFree(d_geo_ub);
+    d_geo_count.release();
+    d_geo_desc.release();
+    d_geo_u32.release();
+    d_geo_dist.release();
+    d_geo_key.release();
     for (auto &ln : lanes) ln.release();
     d_docids_out.release();
     d_sort_desc.release();
@@ -138,6 +145,7 @@ int Engine::stage_finish() {
     try {
         build_host_index(raw_dict_bytes, raw_dict_off, raw_dbs, raw_docids, hix);
         build_sort_fields(raw_dbs[B200_DB_FACET_ID_F64_DOCIDS], raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], hix);
+        build_geo_field(raw_dbs[B200_DB_FACET_ID_F64_DOCIDS], raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], hix);
     } catch (const std::exception &e) {
         return fail(B200_ERR_INVALID, e.what());
     }
@@ -166,6 +174,22 @@ int Engine::stage_finish() {
             stats.hbm_bytes_staged += k.size() * 4;
             std::vector<uint32_t>().swap(k);
         }
+    // GeoSort points: lat_lng_to_xyz (lib.rs:397-404) and cos(lat) with the host's libm, as the reference computes them
+    {
+        GeoField &g = hix.geo;
+        std::vector<GeoPoint> pts(hix.n_docs, GeoPoint{0, 0, 0, 0, 0, 0});
+        const double to_rad = M_PI / 180.0;
+        for (uint32_t d = 0; d < hix.n_docs; d++) {
+            if (!(g.ub[d >> 6] >> (d & 63) & 1)) continue;
+            const double la = g.lat[d] * to_rad, ln = g.lng[d] * to_rad;
+            pts[d] = GeoPoint{std::cos(la) * std::cos(ln), std::cos(la) * std::sin(ln), std::sin(la), g.lat[d], g.lng[d], std::cos(la)};
+        }
+        CU(upload(&d_geo_pts, pts.data(), pts.size()), "upload geo points");
+        CU(upload(&d_geo_ub, reinterpret_cast<const unsigned long long *>(g.ub.data()), g.ub.size()), "upload geo bitmap");
+        stats.hbm_bytes_staged += pts.size() * sizeof(GeoPoint) + g.ub.size() * 8;
+        std::vector<double>().swap(g.lat);
+        std::vector<double>().swap(g.lng);
+    }
     // release the raw staging copies
     for (auto &db : raw_dbs) {
         std::vector<uint8_t>().swap(db.keys);

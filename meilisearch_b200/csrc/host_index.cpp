@@ -1,6 +1,7 @@
 // Staging: decode the LMDB-format databases (keys per heed_codec/*, values per
 // CboRoaringBitmapCodec, crates/milli/src/heed_codec/roaring_bitmap/cbo_roaring_bitmap_codec.rs:15-85)
 // into the HBM posting-store layout described in host_index.h.
+#include <cmath>
 #include "host_index.h"
 
 #include <algorithm>
@@ -370,6 +371,65 @@ void build_sort_fields(const RawDb &f64_db, const RawDb &string_db, HostIndex &i
     };
     fold(nums, true);
     fold(strs, false);
+}
+
+void build_geo_field(const RawDb &f64_db, const RawDb &string_db, HostIndex &ix) {
+    GeoField &g = ix.geo;
+    g.lat.assign(ix.n_docs, 0.0);
+    g.lng.assign(ix.n_docs, 0.0);
+    g.ub.assign(ix.n_words64, 0);
+    g.n_geo = 0;
+    if (g.lat_fid == 0xFFFF || g.lng_fid == 0xFFFF) return;
+    // per coordinate: 0 none, 1 from a number, 2 from a string
+    std::vector<uint8_t> have[2] = {std::vector<uint8_t>(ix.n_docs, 0), std::vector<uint8_t>(ix.n_docs, 0)};
+    std::vector<double> *dst[2] = {&g.lat, &g.lng};
+    const uint16_t fids[2] = {g.lat_fid, g.lng_fid};
+    std::vector<uint32_t> docs;
+    // level-0 entries come in ascending value order per field, so the first value a document meets is its smallest (geo_value
+    // takes the first entry of field_id_docid_facet_{f64s,strings} for (fid, docid), ordered the same way)
+    auto scan = [&](const RawDb &db, bool numbers) {
+        for (uint64_t i = 0; i < db.n; i++) {
+            const uint8_t *k = db.keys.data() + db.koff[i];
+            const size_t kn = db.koff[i + 1] - db.koff[i];
+            if (kn < 3 || k[2] != 0) continue;
+            const uint16_t fid = (uint16_t)(k[0] << 8 | k[1]);
+            for (int c = 0; c < 2; c++) {
+                if (fid != fids[c]) continue;
+                double v = 0;
+                if (numbers) {
+                    if (kn != 3 + 16) throw std::runtime_error("stage: facet_id_f64_docids key without a 16-byte OrderedF64 bound");
+                    uint64_t bits = 0;
+                    for (int b = 0; b < 8; b++) bits = bits << 8 | k[11 + b];
+                    memcpy(&v, &bits, 8);
+                } else {
+                    // str::parse::<f64>: the whole string, no surrounding blanks
+                    std::string str((const char *)k + 3, kn - 3);
+                    char *end = nullptr;
+                    v = str.empty() || isspace((unsigned char)str[0]) || str.find('x') != std::string::npos ? 0.0 : strtod(str.c_str(), &end);
+                    if (!end || *end) v = std::nan("");
+                }
+                docs.clear();
+                cbo_decode_append(db.vals.data() + db.voff[i] + 1, db.voff[i + 1] - db.voff[i] - 1, docs);
+                for (uint32_t d : docs) {
+                    if (d >= ix.n_docs || have[c][d]) continue;
+                    if (!numbers && std::isnan(v))
+                        throw std::runtime_error("stage: a geo coordinate stored as a string does not parse as f64 (docid " + std::to_string(d) + ")");
+                    have[c][d] = numbers ? 1 : 2;
+                    (*dst[c])[d] = v;
+                }
+            }
+        }
+    };
+    scan(f64_db, true);
+    scan(string_db, false);
+    for (uint32_t d = 0; d < ix.n_docs; d++) {
+        if (!have[0][d] && !have[1][d]) continue;
+        if (!have[0][d] || !have[1][d])
+            throw std::runtime_error("stage: document " + std::to_string(d) + " has one geo coordinate without the other");
+        if (!(ix.base_ub[d >> 6] >> (d & 63) & 1)) continue;  // not in documents_ids
+        g.ub[d >> 6] |= 1ull << (d & 63);
+        g.n_geo++;
+    }
 }
 
 }  // namespace b200

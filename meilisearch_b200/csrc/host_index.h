@@ -70,6 +70,16 @@ struct SortField {
     }
 };
 
+// The GeoSort rule's view of the index (documents/geo_sort.rs:252-277): per document its point, from the level-0 entries of the
+// `_geo.lat` / `_geo.lng` fields (number facets first, then strings parsed as f64, the smallest value of each), and the set of
+// documents that have one (geo_faceted_documents_ids).
+struct GeoField {
+    uint16_t lat_fid = 0xFFFF, lng_fid = 0xFFFF;  // 0xFFFF: not staged (no document is geo)
+    std::vector<double> lat, lng;                 // per docid (meaningful where `ub` is set)
+    std::vector<uint64_t> ub;                     // n_words64 words
+    uint64_t n_geo = 0;
+};
+
 struct HostIndex {
     // dictionary
     std::vector<uint8_t> dict_bytes;
@@ -95,6 +105,7 @@ struct HostIndex {
     uint32_t pair_list_base = 0;
     std::map<uint32_t, uint32_t> fwc_list;  // fid<<8|count -> list
     std::map<uint16_t, SortField> sort_fields;  // faceted fields (fid -> SortField)
+    GeoField geo;
     // list id of key i of database db = db_first[db] + i (keys in LMDB order); db_keys[db] = number of staged keys.
     // (word_pair_proximity keys naming unknown words are dropped at staging: for that db the mapping only holds when none was.)
     uint32_t db_first[10] = {0}, db_keys[10] = {0};
@@ -194,5 +205,8 @@ void build_host_index(const std::vector<uint8_t> &dict_bytes, const std::vector<
 // Decode the level-0 entries of facet_id_f64_docids / facet_id_string_docids into out.sort_fields (after build_host_index: needs
 // n_docs).  Throws std::runtime_error on a malformed key or value.
 void build_sort_fields(const RawDb &f64_db, const RawDb &string_db, HostIndex &out);
+// Read every document's point into out.geo (after build_host_index; out.geo.lat_fid / lng_fid set, or nothing to do).  Throws
+// std::runtime_error for a document with one coordinate only or a string coordinate that does not parse as f64.
+void build_geo_field(const RawDb &f64_db, const RawDb &string_db, HostIndex &out);
 
 }  // namespace b200

@@ -29,6 +29,9 @@ cudaError_t launch_walk(cudaStream_t s, int cls, const TileDesc *tiles, uint32_t
 cudaError_t launch_emit(cudaStream_t s, const EmitDesc *emits, uint32_t n_emits);
 // sort.cu: one CTA per window (SortDesc)
 cudaError_t launch_sort_window(cudaStream_t s, const SortDesc *descs, uint32_t n_descs);
+// geo.cu: |universe AND geo| per query (one CTA each); one CTA per window of a GeoSort order (GeoDesc)
+cudaError_t launch_geo_count(cudaStream_t s, const GeoCount *counts, uint32_t n);
+cudaError_t launch_geo_window(cudaStream_t s, const GeoDesc *descs, uint32_t n_descs);
 cudaError_t launch_vec_dist(cudaStream_t s, int n_ctas, int qt, const void *mat_fp16, const float *inv_norm, const uint32_t *docids,
                             uint64_t n_rows, uint32_t d, const float *queries, const float *q_inv_norm, const unsigned long long *cand,
                             uint64_t n_cand_words, float *dist);
