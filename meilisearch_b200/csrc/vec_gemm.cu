@@ -7,13 +7,15 @@
 //
 // Per CTA (one per SM, 256 threads):
 //   warp 0     TMA producer: the query tile [64 x d] once (A operand, resident: d/64 blocks of 8 KB, 128B-swizzled, K-major),
-//              then matrix row tiles [64 rows x 64 halfs] through an 8-stage ring (B operand)
+//              then matrix blocks [128 rows x 64 halfs] = two row tiles through a 4-stage ring (B operand)
 //   warp 1     stages each row tile's docids (filtered rows marked) and inverse norms in shared memory, one tile ahead
 //   warps 2-3  epilogue: lane = query; reads the tile's 64 fp32 dots from the accumulator staging buffer, distance, compare with
 //              the query's running threshold, append survivors to the query's candidate run in L2-resident scratch; a
 //              warp-cooperative bitonic sort compacts a run to its k best whenever it fills up, which tightens the threshold.
-//   warps 4-7  one warpgroup issues wgmma.mma_async m64n64k16 (f16 in, f32 accumulators in registers) over the k-blocks of a row
-//              tile, then writes the accumulators to one of two staging buffers in shared memory for the epilogue
+//   warps 4-7  one warpgroup issues wgmma.mma_async m64n128k16 (f16 in, f32 accumulators in registers) over the k-blocks of two
+//              row tiles, then writes each tile's accumulators to one of two staging buffers in shared memory for the epilogue.
+//              The scan is bound by this loop, not by L2 -> SM delivery (DESIGN.md §4): the wider N halves the instructions
+//              issued and the query-operand bytes read from shared memory per matrix row.
 // CTA c serves query tile c % n_qtiles and the c / n_qtiles-th slice of the row tiles; vec_merge_kernel merges the slices.
 // The query tile is 64 rows (one warpgroup's M) so that a 768-wide tile (96 KB), the matrix ring and the staging buffers fit in
 // the 227 KB of shared memory a block may use.
@@ -32,15 +34,16 @@ namespace b200 {
 namespace {
 
 constexpr int GM = VEC_GEMM_QTILE;  // queries per tile (wgmma M of one warpgroup)
-constexpr int GN = 64;              // matrix rows per tile (wgmma N)
+constexpr int GN = 64;              // matrix rows per tile (the epilogue's unit: row metadata, staging buffer, candidate screen)
+constexpr int MN = 2 * GN;          // matrix rows per MMA (wgmma N): two tiles per instruction
 constexpr int GK = 64;              // halfs per k-block = one 128-byte swizzle span
-constexpr int STAGES = 8;           // B ring depth
+constexpr int STAGES = 4;           // B ring depth (16 KB stages: 64 KB in flight)
 constexpr int NACC = 2;             // accumulator staging buffers
 constexpr int ACC_LD = GM + 4;      // floats per staged column: the fragment stores and the per-query loads are bank-conflict free
 constexpr int META_BUFS = 2;        // row metadata (docid, inverse norm) staged per tile by warp 1
 constexpr int EPI_WARPS = GM / 32;  // epilogue warps, one query per lane
 constexpr int A_BLOCK = GM * GK * 2;        // 8 KB
-constexpr int B_BLOCK = GN * GK * 2;        // 8 KB
+constexpr int B_BLOCK = MN * GK * 2;        // 16 KB
 constexpr int ACC_BYTES = GN * ACC_LD * 4;  // 17 KB
 constexpr int CAND_CAP = VEC_GEMM_CAND_CAP;
 constexpr int KMAX = VEC_GEMM_KMAX;
@@ -106,23 +109,29 @@ __device__ __forceinline__ void wgmma_wait() {
     asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 // keeps the compiler from moving accumulator accesses across the asynchronous MMA
-__device__ __forceinline__ void acc_fence(float (&d)[32]) {
+__device__ __forceinline__ void acc_fence(float (&d)[64]) {
 #pragma unroll
-    for (int i = 0; i < 32; i++) asm volatile("" : "+f"(d[i])::"memory");
+    for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, both operands K-major in shared memory
-__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-        "%32, %33, p, 1, 1, 0, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
-          "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
-          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
-          "+f"(d[31])
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
@@ -253,7 +262,7 @@ __global__ void __launch_bounds__(256, 1)
             for (uint32_t kb = 0; kb < kblocks; kb++) tma_load_2d(sA + (size_t)kb * A_BLOCK, &tmap_q, a_full, (int32_t)(kb * GK), (int32_t)(qtile * GM));
         }
         uint32_t s = 0, ph = 0;
-        for (uint64_t t = tile_lo; t < tile_hi; t++)
+        for (uint64_t t = tile_lo; t < tile_hi; t += 2)
             for (uint32_t kb = 0; kb < kblocks; kb++) {
                 mbar_wait<128>(b_empty + s, ph ^ 1);
                 if (leader) {
@@ -289,16 +298,17 @@ __global__ void __launch_bounds__(256, 1)
             if (lane == 0) mbar_arrive(meta_full + mb);
         }
     } else if (warp >= 4) {
-        // MMA warpgroup: accumulators of a whole row tile in registers (32 fp32 per thread), one commit group per k-block; the ring
-        // stage of k-block kb is released once the group of kb + 1 is issued and that of kb has completed
+        // MMA warpgroup: accumulators of two row tiles in registers (64 fp32 per thread), one commit group per k-block; the ring
+        // stage of k-block kb is released once the group of kb + 1 is issued and that of kb has completed.  An m64n128k16 does the
+        // work of two m64n64k16 in fewer issue slots and shared-memory reads of the query operand; every dot is the same sum.
         const uint32_t wq = warp - 4, g = lane >> 2, q = lane & 3;
         const uint64_t ad0 = make_sdesc(smem_u32(sA)), bd0 = make_sdesc(smem_u32(sB));
         mbar_wait(a_full, 0);
         uint32_t s = 0, ph = 0, n = 0;
-        for (uint64_t t = tile_lo; t < tile_hi; t++, n++) {
-            float acc[32];
+        for (uint64_t t = tile_lo; t < tile_hi; t += 2) {
+            float acc[64];
 #pragma unroll
-            for (int i = 0; i < 32; i++) acc[i] = 0.f;
+            for (int i = 0; i < 64; i++) acc[i] = 0.f;
             uint32_t prev = 0;
             for (uint32_t kb = 0; kb < kblocks; kb++) {
                 mbar_wait(b_full + s, ph);
@@ -306,7 +316,7 @@ __global__ void __launch_bounds__(256, 1)
                 acc_fence(acc);
                 const uint64_t ad = ad0 + (uint64_t)kb * (A_BLOCK >> 4), bd = bd0 + (uint64_t)s * (B_BLOCK >> 4);
 #pragma unroll
-                for (uint32_t k = 0; k < GK / 16; k++) wgmma_m64n64k16(acc, ad + 2 * k, bd + 2 * k, (kb | k) != 0);  // +32 B per K=16 step
+                for (uint32_t k = 0; k < GK / 16; k++) wgmma_m64n128k16(acc, ad + 2 * k, bd + 2 * k, (kb | k) != 0);  // +32 B per K=16 step
                 wgmma_commit();
                 acc_fence(acc);
                 if (kb > 0) {
@@ -322,20 +332,27 @@ __global__ void __launch_bounds__(256, 1)
             wgmma_wait<0>();
             acc_fence(acc);
             if (threadIdx.x == 128) mbar_arrive(b_empty + prev);
-            // fragment -> staging buffer, column-major: element (query r, row c) at c * ACC_LD + r.  Thread (warp wq, lane) holds
-            // queries 16 wq + g and 16 wq + g + 8, rows 8 i + 2 q and 8 i + 2 q + 1 of every n8 block i.
-            const uint32_t buf = n & 1, aph = (n >> 1) & 1;
-            mbar_wait(acc_empty + buf, aph ^ 1);
-            float *dst = sAcc + buf * (ACC_BYTES / 4) + wq * 16 + g;
+            // fragment -> staging buffer, one tile (64 rows) at a time, column-major: element (query r, row c) at c * ACC_LD + r.
+            // Thread (warp wq, lane) holds queries 16 wq + g and 16 wq + g + 8, rows 8 i + 2 q and 8 i + 2 q + 1 of every n8 block i;
+            // blocks 0-7 are tile t, blocks 8-15 tile t + 1.  When the slice has an odd number of tiles, the second half of its last
+            // block (rows of the next slice, or zeros past the matrix) is computed and dropped.
 #pragma unroll
-            for (int i = 0; i < GN / 8; i++) {
-                const uint32_t c = 8 * i + 2 * q;
-                dst[c * ACC_LD] = acc[4 * i];
-                dst[(c + 1) * ACC_LD] = acc[4 * i + 1];
-                dst[c * ACC_LD + 8] = acc[4 * i + 2];
-                dst[(c + 1) * ACC_LD + 8] = acc[4 * i + 3];
+            for (int h = 0; h < MN / GN; h++, n++) {
+                if (t + h >= tile_hi) break;
+                const uint32_t buf = n & 1, aph = (n >> 1) & 1;
+                mbar_wait(acc_empty + buf, aph ^ 1);
+                float *dst = sAcc + buf * (ACC_BYTES / 4) + wq * 16 + g;
+#pragma unroll
+                for (int i = 0; i < GN / 8; i++) {
+                    const uint32_t c = 8 * i + 2 * q;
+                    const int a = 4 * (h * (GN / 8) + i);
+                    dst[c * ACC_LD] = acc[a];
+                    dst[(c + 1) * ACC_LD] = acc[a + 1];
+                    dst[c * ACC_LD + 8] = acc[a + 2];
+                    dst[(c + 1) * ACC_LD + 8] = acc[a + 3];
+                }
+                mbar_arrive(acc_full + buf);
             }
-            mbar_arrive(acc_full + buf);
         }
     } else if (warp >= 2 && warp < 2 + EPI_WARPS) {
         const uint32_t w = warp - 2;
@@ -579,7 +596,7 @@ cudaError_t launch_vec_gemm_topk(cudaStream_t s, uint32_t sm_count, const void *
                                  unsigned long long *partial, uint32_t *out_ids, float *out_dist, uint32_t *out_n, uint32_t n_q) {
     if (!vec_gemm_supported(d, k) || n_qtiles * n_groups > sm_count || n_groups == 0) return cudaErrorInvalidValue;
     CUtensorMap mq, mm;
-    if (!make_map(&mq, q_fp16, (uint64_t)n_qtiles * GM, d, GM) || !make_map(&mm, mat_fp16, n_rows, d, GN)) return cudaErrorNotSupported;
+    if (!make_map(&mq, q_fp16, (uint64_t)n_qtiles * GM, d, GM) || !make_map(&mm, mat_fp16, n_rows, d, MN)) return cudaErrorNotSupported;
     cudaError_t e = cudaMemsetAsync(gthr, 0xff, (size_t)n_qtiles * GM * n_groups * 8, s);
     if (e != cudaSuccess) return e;
     const size_t smem = vec_gemm_smem_bytes(d);
