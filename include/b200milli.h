@@ -216,6 +216,25 @@ typedef struct {
     int32_t geo_strategy;
     uint32_t geo_cache_size;
     uint64_t geo_max_bucket_size;
+    /* Geo filters (IndexFilter::evaluate, search/facet/filter/index_filter.rs:345-360,465-696): the geo leaves at the top of a
+     * query's filter, pushed down.  Query i has clauses [geo_filter_begin[i], geo_filter_begin[i+1]); geo_filter_begin NULL = no geo
+     * filter anywhere.  geo_filter_kind: 0 `_geoRadius(lat, lng, radius)`, 1 `_geoBoundingBox([top, right], [bottom, left])`;
+     * geo_filter_not (NULL = none): 1 = `NOT clause`; geo_filter_args: four doubles per clause, (lat, lng, radius in metres, unused)
+     * or (top, right, bottom, left).  The query's filtered universe is documents_ids AND universes[i] AND every clause, a NOT clause
+     * counting as documents_ids minus the clause.  _geoRadius is the prefix of the rtree order (squared chord distance, ties by
+     * docid) that take_while keeps (haversine <= radius + f64::EPSILON); _geoBoundingBox is the inclusive latitude and longitude
+     * ranges over the staged points, the longitude one wrapping the antimeridian when right < left.  Per query, with the reference's
+     * message: a non-finite argument, a latitude outside [-90, 90], a longitude outside [-180, 180], or top < bottom is
+     * B200_ERR_INVALID, and so is a geo clause when b200_stage_geo_fields was not called (`_geo` not filterable: the message is
+     * `Attribute `_geo/_geojson` is not filterable.`, to which the caller appends the index's filterable patterns as
+     * FilterError::AttributeNotFilterable does).  Every mode takes
+     * the filtered universe exactly as if it had been passed through `universes`.  Queries with the same universe pointer and the
+     * same clause list share one device bitmap; B200_ERR_CAPACITY for the call when the batch's bitmaps do not fit.  GeoJSON
+     * (`_geojson`, `_geoPolygon`, the `resolution` argument) is not implemented. */
+    const uint32_t *geo_filter_begin;
+    const uint8_t *geo_filter_kind;
+    const uint8_t *geo_filter_not;
+    const double *geo_filter_args;
 } b200_query_batch;
 #define B200_MAX_SCORES 12
 /* score kinds: ScoreDetails variants (score_details.rs:9-32) */
@@ -246,6 +265,12 @@ typedef struct {                  /* SearchResult (search/mod.rs:526-535), flatt
 } b200_results;
 int b200_search_batch(b200_index *, const b200_query_batch *, b200_results *);
 
+/* Replaces the geo leaves of IndexFilter::evaluate (index_filter.rs:465-696) inside filter trees the caller combines itself (OR,
+ * nested NOT): clause i (kind[i], args[4 i .. 4 i + 4), as in b200_query_batch::geo_filter_*) becomes the dense bitmap
+ * out[i * out_words ..] (out_words >= ceil((max docid + 1) / 64); words past the document range are zero).  status[i]: 0 or
+ * B200_ERR_INVALID with the reference's message (its bitmap is then empty).  The same kernels as the search batch. */
+int b200_geo_filter_batch(b200_index *, uint32_t n, const uint8_t *kind, const double *args, uint64_t *out, uint64_t out_words, int32_t *status);
+
 /* ---- S1: the RankingRule seam ---------------------------------------------------------- */
 /* Replaces `dyn RankingRule` as driven by bucket_sort (crates/milli/src/search/new/ranking_rules.rs:26-83, bucket_sort.rs:123,266,323)
  * for the graph-based rules and ExactAttribute.  Query graphs are opaque library objects (a QueryGraph plus the terms it refers
@@ -275,7 +300,7 @@ void b200_rule_end(b200_rule *);
 /* kernel classes for the per-kernel accounting below */
 enum b200_kernel { B200_K_LEV = 0, B200_K_COMPACT = 1, B200_K_PAIR_PROBE = 2, B200_K_SCATTER = 3, B200_K_EVAL_PATHS = 4, B200_K_EMIT = 5,
                    B200_K_VEC_DIST = 6, B200_K_TOPK = 7, B200_K_VEC_GEMM = 8, B200_K_VEC_MERGE = 9, B200_K_SORT = 10, B200_K_GEO = 11,
-                   B200_K_COUNT = 12 };
+                   B200_K_GEO_FILTER = 12, B200_K_COUNT = 13 };
 typedef struct {
     uint64_t kernel_launches;     /* kernels launched by the library since the last reset */
     uint64_t device_steps;        /* host<->device round trips since the last reset */

@@ -49,7 +49,8 @@ class _Batch(C.Structure):
                 ("time_budget_ns", C.c_uint64), ("stop_after", C.c_int64), ("has_ranking_score_threshold", C.c_int32),
                 ("ranking_score_threshold", C.c_double), ("sort_begin", C.c_void_p), ("sort_fid", C.c_void_p), ("sort_asc", C.c_void_p),
                 ("sort_geo", C.c_void_p), ("sort_geo_point", C.c_void_p), ("geo_strategy", C.c_int32), ("geo_cache_size", C.c_uint32),
-                ("geo_max_bucket_size", C.c_uint64)]
+                ("geo_max_bucket_size", C.c_uint64), ("geo_filter_begin", C.c_void_p), ("geo_filter_kind", C.c_void_p),
+                ("geo_filter_not", C.c_void_p), ("geo_filter_args", C.c_void_p)]
 
 
 class _Results(C.Structure):
@@ -60,13 +61,13 @@ class _Results(C.Structure):
 
 class _Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("device_steps", C.c_uint64), ("posting_bytes", C.c_uint64), ("matrix_bytes", C.c_uint64),
-                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 12),
-                ("kernel_count", C.c_uint64 * 12), ("kernel_bytes", C.c_uint64 * 12), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
+                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 13),
+                ("kernel_count", C.c_uint64 * 13), ("kernel_bytes", C.c_uint64 * 13), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
                 ("hbm_bytes_staged", C.c_uint64), ("deferred", C.c_uint64), ("arena_peak_bytes", C.c_uint64),
                 ("eval_class_launches", C.c_uint64 * 9), ("eval_class_tiles", C.c_uint64 * 9)]
 
 
-KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort", "geo"]
+KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort", "geo", "geo_filter"]
 
 
 def build_library(force=False):
@@ -110,6 +111,7 @@ def load_library():
         l.b200_comm_unique_id.argtypes = [C.c_void_p, C.c_void_p]
         l.b200_comm_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         l.b200_search_batch.argtypes = [C.c_void_p, C.POINTER(_Batch), C.POINTER(_Results)]
+        l.b200_geo_filter_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
         l.b200_proximity_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
         l.b200_graph_from_tokens.argtypes = [C.c_void_p, C.POINTER(_Batch), C.POINTER(C.c_void_p)]
         l.b200_graph_free.argtypes = [C.c_void_p]
@@ -124,7 +126,7 @@ def load_library():
 
 SYMBOLS = ["b200_open", "b200_close", "b200_last_error", "b200_open_error", "b200_stage_dictionary", "b200_stage_db",
            "b200_stage_documents_ids", "b200_stage_settings", "b200_stage_synonyms", "b200_stage_geo_fields", "b200_stage_finish", "b200_stage_embeddings", "b200_stage_embeddings_f16", "b200_stage_distribution",
-           "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_graph_from_tokens",
+           "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_geo_filter_batch", "b200_graph_from_tokens",
            "b200_graph_free", "b200_rule_start", "b200_rule_next", "b200_rule_end", "b200_get_stats", "b200_reset_stats"]
 
 
@@ -134,6 +136,36 @@ def parse_geo_point(name):
 
     m = re.fullmatch(r"_geoPoint\(\s*([^,\s]+)\s*,\s*([^)\s]+)\s*\)", name)
     return (float(m.group(1)), float(m.group(2))) if m else None
+
+
+# a number as Rust's f64::from_str reads the filter's tokens: sign, digits with an optional fraction and exponent, or inf / infinity /
+# nan in any case (non-finite values are refused by the library with the reference's message)
+_NUM = r"\s*([+-]?(?:(?:\d+\.?\d*|\.\d+)(?:[eE][+-]?\d+)?|(?i:inf|infinity|nan)))\s*"
+_GEO_RADIUS = r"_geoRadius\(" + _NUM + "," + _NUM + "," + _NUM + r"(,.*)?\)"
+_GEO_BOX = r"_geoBoundingBox\(\s*\[" + _NUM + "," + _NUM + r"\]\s*,\s*\[" + _NUM + "," + _NUM + r"\]\s*\)"
+GEO_RADIUS, GEO_BOUNDING_BOX = 0, 1
+
+
+def parse_geo_filter(clause):
+    """(kind, negated, four args) of a geo filter clause: `_geoRadius(lat, lng, radius)` or `_geoBoundingBox([top, right], [bottom,
+    left])`, optionally prefixed by `NOT `, with numbers in Rust's f64 syntax.  Anything else raises ValueError, and so does the `resolution` argument of _geoRadius,
+    which only steers the GeoJSON index (not built here).  Non-finite numbers pass: the library refuses them with the reference's
+    message."""
+    import re
+
+    s = clause.strip()
+    neg = re.match(r"NOT\s+", s)
+    if neg:
+        s = s[neg.end():]
+    m = re.fullmatch(_GEO_RADIUS, s)
+    if m:
+        if m.group(4) is not None:
+            raise ValueError(f"{clause!r}: the resolution argument of _geoRadius is out of scope (GeoJSON filtering is not built)")
+        return GEO_RADIUS, bool(neg), (float(m.group(1)), float(m.group(2)), float(m.group(3)), 0.0)
+    m = re.fullmatch(_GEO_BOX, s)
+    if m:
+        return GEO_BOUNDING_BOX, bool(neg), tuple(float(m.group(i)) for i in range(1, 5))
+    raise ValueError(f"{clause!r} is not a geo filter clause (`[NOT ]_geoRadius(lat, lng, radius)` or `[NOT ]_geoBoundingBox([top, right], [bottom, left])`)")
 
 
 def _p(a):
@@ -392,6 +424,24 @@ class Index:
     def search(self):
         return Search(self)
 
+    def geo_filter(self, clauses):
+        """the geo leaves of a filter tree, one bitmap each (b200_geo_filter_batch): clause strings as Search.geo_filter takes them,
+        without `NOT ` -> (uint64 bitmaps [n, words], statuses [n]); a clause with a non-zero status has an empty bitmap"""
+        parsed = [parse_geo_filter(c) for c in clauses]
+        if any(neg for _, neg, _ in parsed):
+            raise ValueError("Index.geo_filter takes clauses without NOT: complement the bitmap against documents_ids")
+        n = len(parsed)
+        kind = np.asarray([k for k, _, _ in parsed] or [0], np.uint8)
+        args = np.asarray([a for _, _, a in parsed] or [(0.0,) * 4], np.float64).reshape(-1)
+        words = (self._n_docs + 63) // 64
+        out = np.zeros((n, words), np.uint64)
+        status = np.zeros(max(n, 1), np.int32)
+        self._ck(self._l.b200_geo_filter_batch(self._h, n, _p(kind), _p(args), _p(out), words, _p(status)))
+        return out, status[:n]
+
+    def last_error(self):
+        return self._l.b200_last_error(self._h).decode()
+
     def stats(self):
         s = _Stats()
         self._l.b200_get_stats(self._h, C.byref(s))
@@ -470,6 +520,7 @@ class Search:
         self._universes, self._budget_ms, self._stop_after, self._threshold, self._want_candidates = None, None, None, None, False
         self._sort = None
         self._geo_strategy, self._geo_max_bucket = (0, 1000), 1000
+        self._geo_filter = None
 
     def query(self, queries, stop_words=frozenset()):
         self._tokens = queries if isinstance(queries, TokenBatch) else TokenBatch([queries] if isinstance(queries, str) else list(queries), stop_words)
@@ -529,6 +580,12 @@ class Search:
         self._geo_max_bucket = n
         return self
 
+    def geo_filter(self, clauses):
+        """geo leaves at the top of the filter, ANDed with the universe: ["_geoRadius(48.85, 2.35, 2000)", "NOT _geoBoundingBox([1, 2],
+        [0, 1])"] for every query of the batch, or one such list per query (see parse_geo_filter)"""
+        self._geo_filter = clauses
+        return self
+
     def with_candidates(self):
         self._want_candidates = True
         return self
@@ -581,6 +638,18 @@ class Search:
             keep += [begin, fid, asc, is_geo, point]
             b.sort_begin, b.sort_fid, b.sort_asc = _p(begin), _p(fid), _p(asc)
             b.sort_geo, b.sort_geo_point = _p(is_geo), _p(point)
+        if self._geo_filter is not None:
+            gf = self._geo_filter
+            per_q = gf if (gf and isinstance(gf[0], (list, tuple))) else [gf] * n
+            parsed = [[parse_geo_filter(c) for c in x] for x in per_q]
+            begin = np.zeros(n + 1, np.uint32)
+            begin[1:] = np.cumsum([len(x) for x in parsed])
+            flat = [c for x in parsed for c in x]
+            kind = np.asarray([k for k, _, _ in flat] or [0], np.uint8)
+            neg = np.asarray([int(g) for _, g, _ in flat] or [0], np.uint8)
+            args = np.asarray([a for _, _, a in flat] or [(0.0,) * 4], np.float64).reshape(-1)
+            keep += [begin, kind, neg, args]
+            b.geo_filter_begin, b.geo_filter_kind, b.geo_filter_not, b.geo_filter_args = _p(begin), _p(kind), _p(neg), _p(args)
         b.geo_strategy, b.geo_cache_size = self._geo_strategy
         b.geo_max_bucket_size = self._geo_max_bucket
         b.time_budget_ns = 0 if self._budget_ms is None else max(1, int(self._budget_ms * 1e6))

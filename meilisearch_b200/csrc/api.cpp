@@ -280,6 +280,13 @@ int b200_search_batch(b200_index *h, const b200_query_batch *b, b200_results *r)
         return h->e.search_batch(b, r);
     });
 }
+int b200_geo_filter_batch(b200_index *h, uint32_t n, const uint8_t *kind, const double *args, uint64_t *out, uint64_t out_words, int32_t *status) {
+    return guarded(h, [&]() -> int {
+        std::lock_guard<std::mutex> g(h->e.mu);
+        if (!h->e.staged) return h->e.fail(B200_ERR_STATE, "geo filter before b200_stage_finish");
+        return h->e.geo_filter_batch(n, kind, args, out, out_words, status);
+    });
+}
 int b200_get_stats(b200_index *h, b200_stats *out) {
     std::lock_guard<std::mutex> g(h->e.mu);
     *out = h->e.stats;
@@ -314,15 +321,22 @@ int Engine::semantic_batch(const b200_query_batch *b, b200_results *r, uint32_t 
     std::vector<uint32_t> ids((size_t)b->n_queries * k), n(b->n_queries);
     std::vector<float> dist((size_t)b->n_queries * k);
     std::vector<uint64_t> n_cand(b->n_queries, hix.n_documents);
-    if (!b->universes) {
+    const GeoFiltered *gf = geo_filtered;  // queries with geo clauses scan their device bitmap; refused ones are answered below
+    if (!b->universes && !gf) {
         int rc = nns_batch(b->vectors, b->n_queries, emb_d_user, k, nullptr, 0, ids.data(), dist.data(), n.data());
         if (rc != B200_OK) return rc;
     } else {
         // filtered_universe restricts the vector candidates (vector_sort.rs:58-78: `vector_candidates & universe`): the queries
-        // are grouped by bitmap and every group is one scan with that candidate filter
-        if (b->n_universe_words < hix.n_words64) return fail(B200_ERR_INVALID, "universe bitmaps shorter than the document range");
-        std::map<const uint64_t *, std::vector<uint32_t>> groups;
-        for (uint32_t q = 0; q < b->n_queries; q++) groups[b->universes[q]].push_back(q);
+        // are grouped by bitmap (the caller's, or a geo-filtered one on the device) and every group is one scan with that filter
+        if (b->universes && b->n_universe_words < hix.n_words64) return fail(B200_ERR_INVALID, "universe bitmaps shorter than the document range");
+        std::map<std::pair<const uint64_t *, const unsigned long long *>, std::vector<uint32_t>> groups;
+        for (uint32_t q = 0; q < b->n_queries; q++) {
+            if (gf && gf->status[q]) continue;
+            if (gf && gf->d_univ[q])
+                groups[{nullptr, gf->d_univ[q]}].push_back(q);
+            else
+                groups[{b->universes ? b->universes[q] : nullptr, nullptr}].push_back(q);
+        }
         const uint32_t d = emb_d_user;
         for (auto &g : groups) {
             const uint32_t m = (uint32_t)g.second.size();
@@ -330,12 +344,16 @@ int Engine::semantic_batch(const b200_query_batch *b, b200_results *r, uint32_t 
             for (uint32_t i = 0; i < m; i++) memcpy(vq.data() + (size_t)i * d, b->vectors + (size_t)g.second[i] * d, (size_t)d * 4);
             std::vector<uint32_t> gi((size_t)m * k), gn(m);
             std::vector<float> gd((size_t)m * k);
+            const uint64_t *hu = g.first.first;
+            const unsigned long long *du = g.first.second;
             uint64_t cnt = hix.n_documents;
-            if (g.first) {
+            if (du) {
+                cnt = gf->count[g.second[0]];
+            } else if (hu) {
                 cnt = 0;
-                for (uint64_t w = 0; w < hix.n_words64; w++) cnt += (uint64_t)__builtin_popcountll(g.first[w] & hix.base_ub[w]);
+                for (uint64_t w = 0; w < hix.n_words64; w++) cnt += (uint64_t)__builtin_popcountll(hu[w] & hix.base_ub[w]);
             }
-            int rc = nns_batch(vq.data(), m, d, k, g.first, g.first ? hix.n_words64 : 0, gi.data(), gd.data(), gn.data());
+            int rc = nns_batch(vq.data(), m, d, k, hu, hu || du ? hix.n_words64 : 0, gi.data(), gd.data(), gn.data(), false, du);
             if (rc != B200_OK) return rc;
             for (uint32_t i = 0; i < m; i++) {
                 const uint32_t q = g.second[i];
@@ -348,9 +366,22 @@ int Engine::semantic_batch(const b200_query_batch *b, b200_results *r, uint32_t 
     }
     // VectorSort's last bucket (vector_sort.rs:128-160): once the embedded candidates are exhausted, the rest of the universe
     // follows in docid order with `similarity: None`
+    // a geo-filtered universe comes back to the host only when a query's embedded candidates run out, once per slot
+    std::map<const unsigned long long *, std::vector<uint64_t>> geo_u;
     for (uint32_t q = 0; q < b->n_queries; q++) {
-        if (n[q] >= k) continue;
+        if (n[q] >= k || (gf && gf->status[q])) continue;
         const uint64_t *u = b->universes ? b->universes[q] : nullptr;
+        if (gf && gf->d_univ[q]) {
+            std::vector<uint64_t> &h = geo_u[gf->d_univ[q]];
+            if (h.empty()) {
+                h.resize(hix.n_words64);
+                cudaError_t e = cudaMemcpyAsync(h.data(), gf->d_univ[q], hix.n_words64 * 8, cudaMemcpyDeviceToHost, vt.stream);
+                if (e == cudaSuccess) e = cudaStreamSynchronize(vt.stream);
+                if (e != cudaSuccess) return cuda_fail(e, "D2H geo universe");
+                vstats.d2h_bytes += hix.n_words64 * 8;
+            }
+            u = h.data();
+        }
         for (uint64_t w = 0; w < hix.n_words64 && n[q] < k; w++) {
             uint64_t bits = hix.base_ub[w] & (u ? u[w] : ~0ull) & ~(w < emb_bitmap.size() ? emb_bitmap[w] : 0ull);
             while (bits && n[q] < k) {
@@ -450,6 +481,22 @@ int compare_scores(const Hit &l, float lr, const Hit &r, float rr) {  // hybrid.
 
 // Search::execute_hybrid (search/hybrid.rs:264-366)
 int Engine::search_batch(const b200_query_batch *b, b200_results *r) {
+    if (!b->geo_filter_begin) return search_batch_filtered(b, r);
+    // geo filters: every query's filtered universe is computed once, before the modes split (hybrid runs both stages on it)
+    cudaError_t e = cudaSetDevice(device);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaSetDevice");
+    GeoFiltered gf;
+    int rc = geo_filter_universes(b, gf);
+    if (rc != B200_OK) return rc;
+    struct Scope {
+        const GeoFiltered *&p;
+        ~Scope() { p = nullptr; }
+    } scope{geo_filtered};
+    geo_filtered = &gf;
+    return search_batch_filtered(b, r);
+}
+
+int Engine::search_batch_filtered(const b200_query_batch *b, b200_results *r) {
     if (b->mode == 0) return keyword_batch(b, r, b->offset, b->limit, b->scoring_strategy);
     if (b->has_ranking_score_threshold || b->time_budget_ns || b->stop_after >= 0 || r->candidates)
         return fail(B200_ERR_UNSUPPORTED, "ranking-score threshold, deadlines and the candidates bitmap are implemented for keyword searches (mode 0) only");
@@ -461,6 +508,13 @@ int Engine::search_batch(const b200_query_batch *b, b200_results *r) {
         // the criteria lack `sort` is SortRankingRuleMissing (check_sort_criteria, :998-1016), as in keyword searches.
         if (rc1 == B200_OK)
             for (uint32_t q = 0; q < b->n_queries; q++) {
+                if (geo_filtered && geo_filtered->status[q]) {  // a bad geo clause (the vector stage skipped the query)
+                    last_error = geo_filtered->error[q];
+                    r->n_hits[q] = 0;
+                    if (r->status) r->status[q] = geo_filtered->status[q];
+                    if (r->n_candidates) r->n_candidates[q] = 0;
+                    continue;
+                }
                 std::vector<SortRule> unused;
                 const char *why = nullptr;
                 const int code = sort_rules(b, q, true, false, unused, why);

@@ -193,5 +193,31 @@ struct GeoCount {
     uint32_t *out;
 };
 
+// ---- geo filters (geo_filter.cu): _geoRadius / _geoBoundingBox clauses over the staged points
+constexpr uint32_t GEO_FILTER_TILE_WORDS = 16;  // 64-document words one CTA stages in shared memory
+constexpr uint32_t GEO_FILTER_SLOT_CHUNK = 1024; // slots whose counts one CTA accumulates in shared memory at a time
+struct GeoClause {
+    uint32_t kind;        // 0 _geoRadius, 1 _geoBoundingBox
+    uint32_t neg;         // NOT clause
+    // radius: the rtree target lat_lng_to_xyz(base), the haversine target, radius + f64::EPSILON, and squared-chord bounds: a point
+    // with d2 < lo is within the radius, one with d2 > hi beyond it, the haversine decides in between (geo_filter.cu)
+    double q[3];
+    double t_lat, t_lng, t_cos_lat;
+    double r_eps, lo, hi;
+    double top, right, bottom, left;  // bounding box, degrees
+};
+// the first point of the rtree order whose haversine exceeds the radius: (squared distance bits, docid); all ones = none
+struct __align__(16) GeoFirst {
+    unsigned long long key, doc;
+};
+// one filtered universe: ub AND the clauses slot_clauses[c_begin, c_end) (NOT clauses complemented), written to dst, its popcount
+// added to *count
+struct GeoSlot {
+    const unsigned long long *ub;
+    unsigned long long *dst;
+    unsigned long long *count;
+    uint32_t c_begin, c_end;
+};
+
 }  // namespace b200
 

@@ -437,6 +437,13 @@ struct Engine {
     DevBuf<uint32_t> d_geo_u32;
     DevBuf<double> d_geo_dist;
     DevBuf<unsigned long long> d_geo_key;
+    // geo filters (geo_filter.cu, engine_geo.cpp): the distinct clauses, their first failing points, clause ids, slots and counts;
+    // the callers' universes AND documents_ids; the slots' bitmaps (n_words64 words each)
+    DevBuf<GeoClause> d_gf_clause;
+    DevBuf<GeoFirst> d_gf_first;
+    DevBuf<uint32_t> d_gf_u32;
+    DevBuf<GeoSlot> d_gf_slot;
+    DevBuf<unsigned long long> d_gf_count, d_gf_caller, d_gf_univ;
     DevBuf<unsigned long long> d_universes;  // the batch's distinct filtered universes (documents_ids & filter), n_words64 words each
     DevBuf<uint32_t> d_rowtab;      // n_queries x n_words64: word -> (tag, row) of the query's current activation (ActDesc::row_tab)
     // lev buffers
@@ -476,8 +483,9 @@ struct Engine {
                      uint32_t *n_one, uint32_t *two_out, uint32_t *n_two);
     // sharded: every rank passes the same queries and scans its own rows; the per-shard top-k lists are all-gathered (NCCL, on the
     // vector stream) and merged on the device; every rank returns the merged result
+    // dev_cand: a candidate bitmap already on the device (then `cand` is ignored)
     int nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t limit, const uint64_t *cand, uint64_t n_cand_words, uint32_t *ids_out,
-                  float *dist_out, uint32_t *n_out, bool sharded = false);
+                  float *dist_out, uint32_t *n_out, bool sharded = false, const unsigned long long *dev_cand = nullptr);
     ShardComm sc;
     DevBuf<float> d_vpart_dist;  // sliced top-k selection: per-slice candidates
     DevBuf<uint32_t> d_vpart_ids, d_vpart_n;
@@ -486,6 +494,7 @@ struct Engine {
     int comm_load();
     int comm_init(int rank, int world, const uint8_t *unique_id);
     int search_batch(const b200_query_batch *b, b200_results *r);
+    int search_batch_filtered(const b200_query_batch *b, b200_results *r);  // after the geo filters
     int union_postings(int db, const uint32_t *key_index, uint32_t n_keys, const uint64_t *universe, uint64_t n_universe_words, uint64_t *out);
     DevBuf<uint8_t> d_s2;  // S2 scratch: universe | column | ActDesc | jobs | counters
     int keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t offset, uint32_t limit, int scoring);
@@ -498,6 +507,21 @@ struct Engine {
     int proximity_pairs(const uint32_t *left, uint32_t n_left, const uint32_t *right, uint32_t n_right, uint32_t fwd_prox, uint32_t bwd_prox,
                         const uint64_t *universe, uint64_t n_universe_words, uint64_t *out);
     int semantic_batch(const b200_query_batch *b, b200_results *r, uint32_t offset, uint32_t limit);
+    // geo filters (engine_geo.cpp).  search_batch computes every query's geo-filtered universe once, before the dispatch by mode, and
+    // points geo_filtered at the result for the duration of the call; the keyword and vector stages read it.
+    struct GeoFiltered {
+        std::vector<const unsigned long long *> d_univ;  // per query: its filtered universe on the device, nullptr = no geo clause
+        std::vector<uint64_t> count;                     // its cardinality
+        std::vector<int32_t> status;                     // B200_ERR_INVALID: a bad clause, or geo not filterable
+        std::vector<std::string> error;
+    };
+    const GeoFiltered *geo_filtered = nullptr;
+    bool geo_filterable() const;  // b200_stage_geo_fields named both fields
+    int reserve_geo_bitmaps(DevBuf<unsigned long long> &buf, size_t n_bitmaps);  // B200_ERR_CAPACITY when they do not fit
+    int run_geo_filter(const std::vector<GeoClause> &clauses, const std::vector<uint32_t> &slot_clauses, std::vector<GeoSlot> &slots,
+                       std::vector<uint64_t> &counts);
+    int geo_filter_universes(const b200_query_batch *b, GeoFiltered &out);
+    int geo_filter_batch(uint32_t n, const uint8_t *kind, const double *args, uint64_t *out, uint64_t out_words, int32_t *status);
     ~Engine();
 };
 

@@ -1856,7 +1856,7 @@ struct KeywordBatch {
             if (b->n_universe_words < W) return fail(B200_ERR_INVALID, "universe bitmaps shorter than the document range");
             std::map<const uint64_t *, uint32_t> slot_of;
             for (uint32_t i = 0; i < NQ; i++)
-                if (b->universes[i]) slot_of.emplace(b->universes[i], 0);
+                if (b->universes[i] && !geo_universe(i)) slot_of.emplace(b->universes[i], 0);
             uint32_t ns = 0;
             for (auto &kv : slot_of) kv.second = ns++;
             CU(eng.d_universes.reserve((size_t)std::max(1u, ns) * W), "alloc universes");
@@ -1872,16 +1872,30 @@ struct KeywordBatch {
                 stats.h2d_bytes += W * 8;
             }
             for (uint32_t i = 0; i < NQ; i++)
-                if (b->universes[i]) {
+                if (b->universes[i] && !geo_universe(i)) {
                     uint32_t sl = slot_of[b->universes[i]];
                     qs[i]->d_univ = eng.d_universes.p + (size_t)sl * W;
                     qs[i]->univ_count = counts[sl];
                 }
         }
+        // geo filters (Engine::geo_filter_universes): the query's universe already holds its caller's bitmap and clauses
+        if (const Engine::GeoFiltered *gf = eng.geo_filtered)
+            for (uint32_t i = 0; i < NQ; i++) {
+                QState &q = *qs[i];
+                if (gf->status[i] && !q.done) {
+                    q.status = gf->status[i];
+                    q.error = gf->error[i];
+                    q.done = true;
+                } else if (gf->d_univ[i]) {
+                    q.d_univ = gf->d_univ[i];
+                    q.univ_count = gf->count[i];
+                }
+            }
         for (uint32_t i = 0; i < NQ; i++)
             if (!qs[i]->d_univ) qs[i]->univ_count = hix.n_documents;
         return B200_OK;
     }
+    bool geo_universe(uint32_t i) const { return eng.geo_filtered && (eng.geo_filtered->d_univ[i] || eng.geo_filtered->status[i]); }
     // ---- phase 2 (per wave, see drive_waves): typo derivations for every term of queries [lo, hi) in one device sweep
     int derive_range(uint32_t lo, uint32_t hi) {
         auto t_ph = clk::now();

@@ -98,6 +98,13 @@ Engine::~Engine() {
     d_geo_u32.release();
     d_geo_dist.release();
     d_geo_key.release();
+    d_gf_clause.release();
+    d_gf_first.release();
+    d_gf_u32.release();
+    d_gf_slot.release();
+    d_gf_count.release();
+    d_gf_caller.release();
+    d_gf_univ.release();
     for (auto &ln : lanes) ln.release();
     d_docids_out.release();
     d_sort_desc.release();
@@ -371,7 +378,7 @@ int Engine::comm_init(int rank, int world, const uint8_t *unique_id) {
 }
 
 int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t limit, const uint64_t *cand, uint64_t n_cand_words,
-                      uint32_t *ids_out, float *dist_out, uint32_t *n_out, bool sharded) {
+                      uint32_t *ids_out, float *dist_out, uint32_t *n_out, bool sharded, const unsigned long long *dev_cand) {
     if (sharded && (!sc.comm || sc.world < 1)) return fail(B200_ERR_STATE, "sharded nns before b200_comm_init");
     CU(cudaSetDevice(device), "cudaSetDevice");
     if (!dix.emb) return fail(B200_ERR_STATE, "nns before b200_stage_embeddings");
@@ -379,7 +386,7 @@ int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t l
     if (d != dix.emb_d) {  // rows were zero-padded at staging: pad the queries the same way
         std::vector<float> padded((size_t)n_q * dix.emb_d, 0.f);
         for (uint32_t q = 0; q < n_q; q++) memcpy(padded.data() + (size_t)q * dix.emb_d, queries + (size_t)q * d, (size_t)d * 4);
-        return nns_batch(padded.data(), n_q, dix.emb_d, limit, cand, n_cand_words, ids_out, dist_out, n_out, sharded);
+        return nns_batch(padded.data(), n_q, dix.emb_d, limit, cand, n_cand_words, ids_out, dist_out, n_out, sharded, dev_cand);
     }
     if (n_q == 0) return B200_OK;
     const uint64_t N = dix.emb_n;
@@ -391,8 +398,8 @@ int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t l
     CU(d_vsel_dist.reserve((size_t)chunk * (limit + tie_cap)), "alloc selection");
     CU(d_vsel_ids.reserve((size_t)chunk * (limit + tie_cap)), "alloc selection");
     CU(d_vsel_n.reserve((size_t)chunk * 2), "alloc selection");
-    const unsigned long long *d_c = nullptr;
-    if (cand) {
+    const unsigned long long *d_c = dev_cand;
+    if (!d_c && cand) {
         CU(d_cand.reserve(n_cand_words), "alloc candidates");
         CU(cudaMemcpyAsync(d_cand.p, cand, n_cand_words * 8, cudaMemcpyHostToDevice, vt.stream), "H2D candidates");
         d_c = d_cand.p;

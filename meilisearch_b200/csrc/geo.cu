@@ -6,34 +6,16 @@
 //   rtree:     squared Euclidean distance between lat_lng_to_xyz of the point and of the target (its antipode when descending), as
 //              rstar's nearest_neighbor_iter ranks points (((dx*dx) + dy*dy) + dz*dz); ties by docid;
 //   iterative: floor of the haversine distance (geoutils, R = 6371000 m), a stable sort by docid; reversed when descending.
-// Points and cos(lat) are staged as computed by the host's libm; the squared distance is rounded exactly as on the host (no fused
-// multiply-add), so rtree keys are bit-identical.  The haversine uses the device's sin / atan2 (within a few ULP of the host's).
+// The distances are those of geo_math.cuh.
 #include <cuda_runtime.h>
 
 #include "device_types.h"
+#include "geo_math.cuh"
 #include "tuple_select.cuh"
 
 namespace b200 {
 
 namespace {
-
-constexpr double EARTH_RADIUS_M = 6371000.0;
-
-// Location::haversine_distance_to (geoutils), from the target (t) to the point (p).  sin(to_radians(d) / 2) is taken as
-// sinpi(d / 360): both are within a few ULP of the true value, and sinpi needs no slow-path argument reduction (a call that
-// spills registers).
-__device__ __forceinline__ double haversine_m(double t_lat, double t_lng, double t_cos_lat, const GeoPoint &p) {
-    const double s_lat = sinpi(__ddiv_rn(__dsub_rn(p.lat, t_lat), 360.0)), s_lng = sinpi(__ddiv_rn(__dsub_rn(p.lng, t_lng), 360.0));
-    const double a = __dadd_rn(__dmul_rn(s_lat, s_lat), __dmul_rn(__dmul_rn(__dmul_rn(s_lng, s_lng), t_cos_lat), p.cos_lat));
-    const double c = __dmul_rn(2.0, atan2(__dsqrt_rn(a), __dsqrt_rn(__dsub_rn(1.0, a))));
-    return __dmul_rn(c, EARTH_RADIUS_M);
-}
-
-__device__ __forceinline__ unsigned long long rtree_key(const double *q, const GeoPoint &p) {
-    const double dx = __dsub_rn(p.x, q[0]), dy = __dsub_rn(p.y, q[1]), dz = __dsub_rn(p.z, q[2]);
-    const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
-    return (unsigned long long)__double_as_longlong(d2);  // >= 0: the bits order as the values
-}
 
 __device__ __forceinline__ uint32_t floor_m(double m) { return (uint32_t)min(m, (double)GEO_FLOOR_MAX); }
 

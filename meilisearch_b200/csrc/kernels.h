@@ -32,6 +32,12 @@ cudaError_t launch_sort_window(cudaStream_t s, const SortDesc *descs, uint32_t n
 // geo.cu: |universe AND geo| per query (one CTA each); one CTA per window of a GeoSort order (GeoDesc)
 cudaError_t launch_geo_count(cudaStream_t s, const GeoCount *counts, uint32_t n);
 cudaError_t launch_geo_window(cudaStream_t s, const GeoDesc *descs, uint32_t n_descs);
+// geo_filter.cu: pass 1, the first failing point of every radius clause in `radius` (first[] all ones at launch); pass 2, the slots
+// (counts zero at launch).  Both stage GEO_FILTER_TILE_WORDS words of points per CTA and loop over the clauses / slots.
+cudaError_t launch_geo_first_fail(cudaStream_t s, const unsigned long long *geo, const GeoPoint *pts, uint32_t n_words, const GeoClause *clauses,
+                                  const uint32_t *radius, uint32_t n_radius, GeoFirst *first);
+cudaError_t launch_geo_filter(cudaStream_t s, const unsigned long long *geo, const GeoPoint *pts, uint32_t n_words, const GeoClause *clauses,
+                              const GeoFirst *first, const uint32_t *slot_clauses, const GeoSlot *slots, uint32_t n_slots);
 cudaError_t launch_vec_dist(cudaStream_t s, int n_ctas, int qt, const void *mat_fp16, const float *inv_norm, const uint32_t *docids,
                             uint64_t n_rows, uint32_t d, const float *queries, const float *q_inv_norm, const unsigned long long *cand,
                             uint64_t n_cand_words, float *dist);
