@@ -79,6 +79,9 @@ class FacetImage:
         self.fields = {}  # name -> fid
         self.numbers = {}  # fid -> {float: [docids]}
         self.strings = {}  # fid -> {normalised str: [docids]}
+        # (fid, docid, normalised str) -> original string, what field_id_docid_facet_strings holds.  A document can give one normalised
+        # value several originals ("Blue" and "blue " in one array); the first one it gives is kept.
+        self.originals = {}
 
     def fid(self, name):
         if name not in self.fields:
@@ -92,6 +95,7 @@ class FacetImage:
             v = normalize_facet(value)
             if v:
                 self.strings.setdefault(f, {}).setdefault(v, []).append(docid)
+                self.originals.setdefault((f, docid, v), value)
         else:
             self.numbers.setdefault(f, {}).setdefault(float(value), []).append(docid)
 
@@ -179,6 +183,9 @@ class FacetImage:
         for v, a, b in zip(vals, starts, ends):
             key = float(v) if numbers else normalize_facet(str(v))
             tab.setdefault(key, []).extend(int(x) for x in docids[order[a:b]])
+            if not numbers:
+                for x in docids[order[a:b]]:
+                    self.originals.setdefault((f, int(x), key), str(v))
 
     def build(self):
         """-> (facet_id_f64_docids, facet_id_string_docids) as DbImage, keys in LMDB (bytewise) order"""

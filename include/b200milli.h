@@ -235,6 +235,22 @@ typedef struct {
     const uint8_t *geo_filter_kind;
     const uint8_t *geo_filter_not;
     const double *geo_filter_args;
+    /* The `facets` search parameter (crates/meilisearch/src/search/mod.rs:1945-1952,2041-2124): FacetDistribution::execute and
+     * compute_stats (search/facet/facet_distribution.rs:110-337, facet_distribution_iter.rs:26-232) over the query's
+     * SearchResult::candidates, on the device.  Query i asks for slots [facet_begin[i], facet_begin[i+1]), slot k for the field
+     * facet_fid[k] (its id in the facet databases; the caller resolves the names against the filterable rules, as
+     * compute_facet_distribution_stats does, and a fid without facet values gives an empty distribution and no stats); facet_begin
+     * NULL = no facets anywhere.  facet_order (NULL = all alpha): 0 OrderBy::Lexicographic, 1 OrderBy::Count (B200_ERR_UNSUPPORTED for
+     * that query).  facet_max_values: maxValuesPerFacet (0 is legal and keeps the reference's meaning).  facet_cap: entries per slot
+     * in the b200_results::facet_* outputs; a slot that needs more fails its query alone with B200_ERR_CAPACITY (max_values + the
+     * field's number of string values always suffices when max_values > 0, the field's number of values when it is 0).
+     * Per query: facets in mode 1 or 2 (use b200_facet_distribution_batch) or with a ranking-score threshold are B200_ERR_UNSUPPORTED;
+     * a facet_begin without facet_fid or without the facet_* outputs is B200_ERR_INVALID. */
+    const uint32_t *facet_begin;
+    const uint16_t *facet_fid;
+    const uint8_t *facet_order;
+    uint32_t facet_max_values;
+    uint32_t facet_cap;
 } b200_query_batch;
 #define B200_MAX_SCORES 12
 /* score kinds: ScoreDetails variants (score_details.rs:9-32) */
@@ -262,6 +278,29 @@ typedef struct {                  /* SearchResult (search/mod.rs:526-535), flatt
     uint64_t *candidates;         /* optional (may be NULL): n_queries x candidates_words dense u64 words, SearchResult::candidates
                                      for keyword searches without a ranking-score threshold (others: B200_ERR_UNSUPPORTED) */
     uint64_t candidates_words;    /* words per query in `candidates` (>= ceil((max docid + 1) / 64)) */
+    /* Facets of slot k (b200_query_batch::facet_*), over exactly the bitmap `candidates` holds for the query.  The distribution
+     * comes as facet_n_num[k] number entries then facet_n_str[k] string entries at [k * facet_cap, ..), each already in the
+     * reference's order and cut to the reference's length (facet_values, facet_distribution.rs:258-294):
+     *   |candidates| <= 3000 (from documents, :110-177): up to max_values numbers in the order of their f64 Display strings, then up
+     *     to max_values - n_num strings in byte order of their normalised value;
+     *   |candidates| > 3000 (facet levels, :181-253): numbers ascending, up to max_values of them (all when max_values is 0), then
+     *     strings in byte order, up to max_values of them when n_num < max_values, all of them otherwise.
+     * The caller builds the IndexMap<String, u64>: insert the numbers (key: the value's f64 Display string), then the strings one by one
+     * (key: the original string of (fid, facet_docid, normalised value) in field_id_docid_facet_strings), stopping right after an
+     * insert that leaves the map's length at max_values.  That reproduces both paths including a string whose original equals a
+     * number's Display string (it overwrites that entry in place).
+     * facet_key: the value's position among the staged level-0 keys of its database (facet_id_f64_docids for the first n_num
+     * entries, facet_id_string_docids after them), as B200_S_SORT's score_rank; facet_count: |candidates AND docids(value)|;
+     * facet_docid: the smallest candidate holding the value (any_docid).  facet_has_stats / facet_min / facet_max: compute_stats
+     * (:298-337, facet/mod.rs:39-59), the smallest and largest number value of the field over the candidates (has_stats 0: none). */
+    uint32_t *facet_n_num;
+    uint32_t *facet_n_str;
+    uint32_t *facet_key;
+    uint64_t *facet_count;
+    uint32_t *facet_docid;
+    uint8_t *facet_has_stats;
+    double *facet_min;
+    double *facet_max;
 } b200_results;
 int b200_search_batch(b200_index *, const b200_query_batch *, b200_results *);
 
@@ -270,6 +309,17 @@ int b200_search_batch(b200_index *, const b200_query_batch *, b200_results *);
  * out[i * out_words ..] (out_words >= ceil((max docid + 1) / 64); words past the document range are zero).  status[i]: 0 or
  * B200_ERR_INVALID with the reference's message (its bitmap is then empty).  The same kernels as the search batch. */
 int b200_geo_filter_batch(b200_index *, uint32_t n, const uint8_t *kind, const double *args, uint64_t *out, uint64_t out_words, int32_t *status);
+
+/* Replaces FacetDistribution::execute and compute_stats (search/facet/facet_distribution.rs:110-337) for callers that hold the
+ * candidates themselves (semantic and hybrid searches, the S1 seam, federated search): candidate set i is the host bitmap
+ * candidates[i] (dense little-endian u64 words, n_words >= ceil((max docid + 1) / 64); only docids below max docid + 1 are read;
+ * equal pointers are uploaded once) and asks for slots [facet_begin[i], facet_begin[i+1]) of facet_fid / facet_order, as in
+ * b200_query_batch.  The outputs are b200_results::facet_* with stride `cap`; status[i]: 0, B200_ERR_UNSUPPORTED (count order) or
+ * B200_ERR_CAPACITY (a slot needs more than `cap` entries), for that set alone.  The same kernels as the search batch. */
+int b200_facet_distribution_batch(b200_index *, uint32_t n, const uint64_t *const *candidates, uint64_t n_words, const uint32_t *facet_begin,
+                                  const uint16_t *facet_fid, const uint8_t *facet_order, uint32_t max_values, uint32_t cap, uint32_t *n_num,
+                                  uint32_t *n_str, uint32_t *key, uint64_t *count, uint32_t *docid, uint8_t *has_stats, double *min,
+                                  double *max, int32_t *status);
 
 /* ---- S1: the RankingRule seam ---------------------------------------------------------- */
 /* Replaces `dyn RankingRule` as driven by bucket_sort (crates/milli/src/search/new/ranking_rules.rs:26-83, bucket_sort.rs:123,266,323)
@@ -300,7 +350,7 @@ void b200_rule_end(b200_rule *);
 /* kernel classes for the per-kernel accounting below */
 enum b200_kernel { B200_K_LEV = 0, B200_K_COMPACT = 1, B200_K_PAIR_PROBE = 2, B200_K_SCATTER = 3, B200_K_EVAL_PATHS = 4, B200_K_EMIT = 5,
                    B200_K_VEC_DIST = 6, B200_K_TOPK = 7, B200_K_VEC_GEMM = 8, B200_K_VEC_MERGE = 9, B200_K_SORT = 10, B200_K_GEO = 11,
-                   B200_K_GEO_FILTER = 12, B200_K_COUNT = 13 };
+                   B200_K_GEO_FILTER = 12, B200_K_FACET = 13, B200_K_COUNT = 14 };
 typedef struct {
     uint64_t kernel_launches;     /* kernels launched by the library since the last reset */
     uint64_t device_steps;        /* host<->device round trips since the last reset */

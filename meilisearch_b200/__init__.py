@@ -50,24 +50,27 @@ class _Batch(C.Structure):
                 ("ranking_score_threshold", C.c_double), ("sort_begin", C.c_void_p), ("sort_fid", C.c_void_p), ("sort_asc", C.c_void_p),
                 ("sort_geo", C.c_void_p), ("sort_geo_point", C.c_void_p), ("geo_strategy", C.c_int32), ("geo_cache_size", C.c_uint32),
                 ("geo_max_bucket_size", C.c_uint64), ("geo_filter_begin", C.c_void_p), ("geo_filter_kind", C.c_void_p),
-                ("geo_filter_not", C.c_void_p), ("geo_filter_args", C.c_void_p)]
+                ("geo_filter_not", C.c_void_p), ("geo_filter_args", C.c_void_p), ("facet_begin", C.c_void_p), ("facet_fid", C.c_void_p),
+                ("facet_order", C.c_void_p), ("facet_max_values", C.c_uint32), ("facet_cap", C.c_uint32)]
 
 
 class _Results(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("docids", "n_hits", "n_scores", "score_kind", "score_rank", "score_max", "score_sim",
                                           "n_candidates", "semantic_hits", "status", "degraded", "used_negative_operator", "candidates")] + \
-               [("candidates_words", C.c_uint64)]
+               [("candidates_words", C.c_uint64)] + \
+               [(n, C.c_void_p) for n in ("facet_n_num", "facet_n_str", "facet_key", "facet_count", "facet_docid", "facet_has_stats", "facet_min",
+                                          "facet_max")]
 
 
 class _Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("device_steps", C.c_uint64), ("posting_bytes", C.c_uint64), ("matrix_bytes", C.c_uint64),
-                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 13),
-                ("kernel_count", C.c_uint64 * 13), ("kernel_bytes", C.c_uint64 * 13), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
+                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 14),
+                ("kernel_count", C.c_uint64 * 14), ("kernel_bytes", C.c_uint64 * 14), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
                 ("hbm_bytes_staged", C.c_uint64), ("deferred", C.c_uint64), ("arena_peak_bytes", C.c_uint64),
                 ("eval_class_launches", C.c_uint64 * 9), ("eval_class_tiles", C.c_uint64 * 9)]
 
 
-KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort", "geo", "geo_filter"]
+KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort", "geo", "geo_filter", "facet"]
 
 
 def build_library(force=False):
@@ -112,6 +115,8 @@ def load_library():
         l.b200_comm_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         l.b200_search_batch.argtypes = [C.c_void_p, C.POINTER(_Batch), C.POINTER(_Results)]
         l.b200_geo_filter_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+        l.b200_facet_distribution_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
+                                                    C.c_uint32] + [C.c_void_p] * 9
         l.b200_proximity_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
         l.b200_graph_from_tokens.argtypes = [C.c_void_p, C.POINTER(_Batch), C.POINTER(C.c_void_p)]
         l.b200_graph_free.argtypes = [C.c_void_p]
@@ -126,7 +131,7 @@ def load_library():
 
 SYMBOLS = ["b200_open", "b200_close", "b200_last_error", "b200_open_error", "b200_stage_dictionary", "b200_stage_db",
            "b200_stage_documents_ids", "b200_stage_settings", "b200_stage_synonyms", "b200_stage_geo_fields", "b200_stage_finish", "b200_stage_embeddings", "b200_stage_embeddings_f16", "b200_stage_distribution",
-           "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_geo_filter_batch", "b200_graph_from_tokens",
+           "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_geo_filter_batch", "b200_facet_distribution_batch", "b200_graph_from_tokens",
            "b200_graph_free", "b200_rule_start", "b200_rule_next", "b200_rule_end", "b200_get_stats", "b200_reset_stats"]
 
 
@@ -172,6 +177,66 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
+FACET_ORDERS = {"alpha": 0, "count": 1}  # OrderBy::Lexicographic / OrderBy::Count (sortFacetValuesBy)
+DEFAULT_VALUES_PER_FACET = 100  # facet_distribution.rs DEFAULT_VALUES_PER_FACET
+
+
+def rust_f64_display(x):
+    """Rust's `impl Display for f64`: the shortest digits that read back as the same value, never an exponent ("-0" for -0.0)"""
+    import decimal
+
+    if x != x:
+        return "NaN"
+    if x in (float("inf"), float("-inf")):
+        return "inf" if x > 0 else "-inf"
+    s = format(decimal.Decimal(repr(float(x))), "f")  # repr: the shortest round-trip digits
+    return s.rstrip("0").rstrip(".") if "." in s else s
+
+
+class _FacetOutputs:
+    """The slots of a facet request and their b200_results::facet_* outputs: per_set holds one list of field names per query (or
+    candidate set); begin / fid / orders are the request's arrays, with `cap` entries per slot"""
+
+    def __init__(self, index, per_set, order, max_values, cap=None):
+        self.begin = np.zeros(len(per_set) + 1, np.uint32)
+        self.begin[1:] = np.cumsum([len(x) for x in per_set])
+        n_slots = int(self.begin[-1])
+        self.fid = np.asarray([index.field_id(x) for p in per_set for x in p] or [0], np.uint16)
+        self.fids = [int(x) for x in self.fid]
+        self.orders = np.full(max(n_slots, 1), FACET_ORDERS[order], np.uint8)
+        cap = index.facet_cap({x for p in per_set for x in p}, max_values) if cap is None else cap
+        n = max(n_slots, 1)
+        self.cap = cap
+        self.n_num = np.zeros(n, np.uint32)
+        self.n_str = np.zeros(n, np.uint32)
+        self.key = np.zeros(max(n * cap, 1), np.uint32)
+        self.count = np.zeros(max(n * cap, 1), np.uint64)
+        self.docid = np.zeros(max(n * cap, 1), np.uint32)
+        self.has_stats = np.zeros(n, np.uint8)
+        self.min = np.zeros(n, np.float64)
+        self.max = np.zeros(n, np.float64)
+
+    def pointers(self):
+        return [_p(a) for a in (self.n_num, self.n_str, self.key, self.count, self.docid, self.has_stats, self.min, self.max)]
+
+    def distribution(self, index, k, max_values):
+        """the reference's IndexMap for slot k, built with the caller's merge rule (b200milli.h): the numbers, keyed by their f64
+        Display string, then the strings one by one, keyed by their original, until an insert leaves the map at max_values entries"""
+        fid = self.fids[k]
+        out = {}
+        at, nn, ns = k * self.cap, int(self.n_num[k]), int(self.n_str[k])
+        for e in range(at, at + nn):
+            out[rust_f64_display(index.sort_value(fid, 0, int(self.key[e]))[1])] = int(self.count[e])
+        for e in range(at + nn, at + nn + ns):
+            out[index.facet_original(fid, int(self.docid[e]), index.sort_value(fid, 1, int(self.key[e]))[1])] = int(self.count[e])
+            if len(out) == max_values:
+                break
+        return list(out.items())
+
+    def stats(self, k):
+        return (float(self.min[k]), float(self.max[k])) if self.has_stats[k] else None
+
+
 class SearchResult:
     """milli::SearchResult (search/mod.rs:526-535) for a batch of queries."""
 
@@ -194,6 +259,18 @@ class SearchResult:
         self.degraded = np.zeros(n, np.uint8)
         self.used_negative_operator = np.zeros(n, np.uint8)
         self.candidates = None  # (n, words) uint64 when requested with Search.with_candidates()
+        self._facets = None  # (index, per query its field names, begin, _FacetOutputs, max values) with Search.facets()
+
+    def facet_distribution(self, q):
+        """facetDistribution of query q: {field name: [(key, count), ...]} in the reference's order"""
+        ix, names, begin, out, mx = self._facets
+        return {name: out.distribution(ix, int(begin[q]) + j, mx) for j, name in enumerate(names[q])}
+
+    def facet_stats(self, q):
+        """facetStats of query q: {field name: (min, max)} over its number values, fields without one left out"""
+        ix, names, begin, out, _ = self._facets
+        st = {name: out.stats(int(begin[q]) + j) for j, name in enumerate(names[q])}
+        return {k: v for k, v in st.items() if v is not None}
 
     def ids(self, q):
         return [int(x) for x in self.documents_ids[q, : self.n_hits[q]]]
@@ -442,6 +519,44 @@ class Index:
     def last_error(self):
         return self._l.b200_last_error(self._h).decode()
 
+    def facet_original(self, fid, docid, normalized):
+        """the original string of a string facet value (field_id_docid_facet_strings at (fid, docid, normalised)), the normalised
+        value when the facet image did not record one (the reference logs an error and does the same)"""
+        orig = getattr(self._facets, "originals", {}) if self._facets is not None else {}
+        return orig.get((fid, docid, normalized), normalized)
+
+    def facet_cap(self, names, max_values):
+        """entries per slot that always suffice: max_values + the field's string values, or all its values when max_values is 0"""
+        f = self._facets
+        cap = 1
+        for name in names:
+            fid = self.field_id(name)
+            n_num, n_str = len(f.numbers.get(fid, {})) if f else 0, len(f.strings.get(fid, {})) if f else 0
+            cap = max(cap, n_num + n_str if max_values == 0 else max_values + n_str)
+        return cap
+
+    def facet_distribution(self, candidates, names, max_values=DEFAULT_VALUES_PER_FACET, order="alpha", cap=None):
+        """FacetDistribution::execute + compute_stats for candidate bitmaps the caller holds (b200_facet_distribution_batch):
+        candidates: a list of uint64 word arrays; names: one list of field names for all, or one per bitmap ->
+        (per bitmap {name: [(key, count), ...]}, per bitmap {name: (min, max)}, statuses)"""
+        n = len(candidates)
+        per = names if (names and isinstance(names[0], (list, tuple))) else [names] * n
+        out = _FacetOutputs(self, per, order, max_values, cap)
+        begin = out.begin
+        cache = {}
+        arrs = [cache.setdefault(id(c), np.ascontiguousarray(c, np.uint64)) for c in candidates]
+        ptrs = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in arrs])
+        words = len(arrs[0]) if arrs else 0
+        status = np.zeros(max(n, 1), np.int32)
+        self._ck(self._l.b200_facet_distribution_batch(self._h, n, C.cast(ptrs, C.c_void_p), words, _p(begin), _p(out.fid), _p(out.orders), max_values,
+                                                       out.cap, *out.pointers(), _p(status)))
+        dists, stats = [], []
+        for i in range(n):
+            ks = range(int(begin[i]), int(begin[i + 1]))
+            dists.append({name: out.distribution(self, k, max_values) for name, k in zip(per[i], ks)})
+            stats.append({name: out.stats(k) for name, k in zip(per[i], ks) if out.stats(k) is not None})
+        return dists, stats, status[:n]
+
     def stats(self):
         s = _Stats()
         self._l.b200_get_stats(self._h, C.byref(s))
@@ -521,6 +636,7 @@ class Search:
         self._sort = None
         self._geo_strategy, self._geo_max_bucket = (0, 1000), 1000
         self._geo_filter = None
+        self._facet_names, self._max_values, self._facet_order, self._facet_cap = None, DEFAULT_VALUES_PER_FACET, "alpha", None
 
     def query(self, queries, stop_words=frozenset()):
         self._tokens = queries if isinstance(queries, TokenBatch) else TokenBatch([queries] if isinstance(queries, str) else list(queries), stop_words)
@@ -584,6 +700,26 @@ class Search:
         """geo leaves at the top of the filter, ANDed with the universe: ["_geoRadius(48.85, 2.35, 2000)", "NOT _geoBoundingBox([1, 2],
         [0, 1])"] for every query of the batch, or one such list per query (see parse_geo_filter)"""
         self._geo_filter = clauses
+        return self
+
+    def facets(self, names):
+        """the `facets` search parameter: field names for every query of the batch, or one such list per query"""
+        self._facet_names = names
+        return self
+
+    def max_values_per_facet(self, n):
+        """maxValuesPerFacet (default 100)"""
+        self._max_values = n
+        return self
+
+    def facet_order(self, order):
+        """sortFacetValuesBy for every field: "alpha" (the default) or "count" (refused by the library)"""
+        self._facet_order = order
+        return self
+
+    def facet_cap(self, cap):
+        """entries per (query, field) in the facet outputs (default: Index.facet_cap, always enough)"""
+        self._facet_cap = cap
         return self
 
     def with_candidates(self):
@@ -659,6 +795,16 @@ class Search:
         r = _Results(_p(res.documents_ids), _p(res.n_hits), _p(res.n_scores), _p(res.score_kind), _p(res.score_rank), _p(res.score_max),
                      _p(res.score_sim), _p(res.n_candidates), _p(res.semantic_hit_count), _p(res.status), _p(res.degraded),
                      _p(res.used_negative_operator), None, 0)
+        if self._facet_names is not None:
+            fn = self._facet_names
+            per_q = [list(x) for x in fn] if (fn and isinstance(fn[0], (list, tuple))) else [list(fn)] * n
+            out = _FacetOutputs(ix, per_q, self._facet_order, self._max_values, self._facet_cap)
+            keep.append(out)
+            b.facet_begin, b.facet_fid, b.facet_order = _p(out.begin), _p(out.fid), _p(out.orders)
+            b.facet_max_values, b.facet_cap = self._max_values, out.cap
+            (r.facet_n_num, r.facet_n_str, r.facet_key, r.facet_count, r.facet_docid, r.facet_has_stats, r.facet_min,
+             r.facet_max) = out.pointers()
+            res._facets = (ix, per_q, out.begin, out, self._max_values)
         if self._want_candidates:
             words = (ix._n_docs + 63) // 64
             res.candidates = np.zeros((n, words), np.uint64)

@@ -287,6 +287,25 @@ int b200_geo_filter_batch(b200_index *h, uint32_t n, const uint8_t *kind, const 
         return h->e.geo_filter_batch(n, kind, args, out, out_words, status);
     });
 }
+int b200_facet_distribution_batch(b200_index *h, uint32_t n, const uint64_t *const *candidates, uint64_t n_words, const uint32_t *facet_begin,
+                                  const uint16_t *facet_fid, const uint8_t *facet_order, uint32_t max_values, uint32_t cap, uint32_t *n_num,
+                                  uint32_t *n_str, uint32_t *key, uint64_t *count, uint32_t *docid, uint8_t *has_stats, double *min,
+                                  double *max, int32_t *status) {
+    return guarded(h, [&]() -> int {
+        std::lock_guard<std::mutex> g(h->e.mu);
+        if (!h->e.staged) return h->e.fail(B200_ERR_STATE, "facet distribution before b200_stage_finish");
+        b200_results dst{};
+        dst.facet_n_num = n_num;
+        dst.facet_n_str = n_str;
+        dst.facet_key = key;
+        dst.facet_count = count;
+        dst.facet_docid = docid;
+        dst.facet_has_stats = has_stats;
+        dst.facet_min = min;
+        dst.facet_max = max;
+        return h->e.facet_distribution_batch(n, candidates, n_words, facet_begin, facet_fid, facet_order, max_values, cap, dst, status);
+    });
+}
 int b200_get_stats(b200_index *h, b200_stats *out) {
     std::lock_guard<std::mutex> g(h->e.mu);
     *out = h->e.stats;
@@ -512,6 +531,13 @@ int Engine::search_batch_filtered(const b200_query_batch *b, b200_results *r) {
                     last_error = geo_filtered->error[q];
                     r->n_hits[q] = 0;
                     if (r->status) r->status[q] = geo_filtered->status[q];
+                    if (r->n_candidates) r->n_candidates[q] = 0;
+                    continue;
+                }
+                if (b->facet_begin && b->facet_begin[q + 1] > b->facet_begin[q]) {
+                    last_error = "facets in a semantic or hybrid search (use b200_facet_distribution_batch over its candidates)";
+                    r->n_hits[q] = 0;
+                    if (r->status) r->status[q] = B200_ERR_UNSUPPORTED;
                     if (r->n_candidates) r->n_candidates[q] = 0;
                     continue;
                 }

@@ -219,5 +219,29 @@ struct GeoSlot {
     uint32_t c_begin, c_end;
 };
 
+// ---- facet distribution (facet.cu): one slot = one (candidate bitmap, faceted field)
+constexpr uint32_t FACET_CANDIDATES_THRESHOLD = 3000;  // facet_distribution.rs:32 CANDIDATES_THRESHOLD
+constexpr uint32_t FACET_SHARED_VALUES = 2048;         // fields with at most this many values count in shared memory
+constexpr uint32_t FACET_ALL = 0xffffffffu;            // "no limit" for the number of entries taken
+// per slot in scratch, zero at launch: |candidates|; the smallest number ordinal met as ~ordinal (atomicMax; 0 = none); the largest
+// plus one (0 = none)
+struct FacetHead {
+    unsigned long long n_cand;
+    uint32_t min_inv, max_p1;
+};
+struct FacetSlot {
+    const unsigned long long *cand;  // candidates: n_words words
+    const uint32_t *doc_off;         // the field's document-major ordinals (SortField), nullptr for a field without values
+    const uint32_t *doc_ord;
+    const uint32_t *disp;            // number ordinals in f64 Display-string order
+    uint32_t n_num, n_str;
+    uint32_t *cnt, *first;           // scratch, zero at launch: per ordinal |candidates AND docids| and ~(smallest such docid)
+    FacetHead *head;
+    uint32_t max_values, cap;
+    uint32_t *out_ord, *out_doc;     // cap entries: numbers first, then strings
+    unsigned long long *out_cnt;
+    uint32_t *out_sum;               // 4 u32: numbers taken, strings taken, FacetHead::min_inv, FacetHead::max_p1
+};
+
 }  // namespace b200
 

@@ -212,6 +212,8 @@ struct Lane {
     DevBuf<uint32_t> d_bigq;  // indices of the step's big scatter jobs (scatter_kernel -> scatter_big_kernel)
     DevBuf<PathOut> d_pathbuf;
     DevBuf<unsigned long long> d_tile_summary;  // 2 u64 per eval tile: its non-empty buckets (eval_dp_kernel -> walk_kernel)
+    DevBuf<uint8_t> d_facet;                    // facet counts of the slots in flight (facet.cu)
+    DevBuf<FacetSlot> d_facet_slots;
     uint8_t *h_step = nullptr;
     size_t h_step_cap = 0;
     uint32_t *h_results = nullptr;
@@ -271,6 +273,8 @@ struct Lane {
         d_pathbuf.release();
         d_tile_summary.release();
         d_bigq.release();
+        d_facet.release();
+        d_facet_slots.release();
         if (h_step) cudaFreeHost(h_step);
         if (h_results) cudaFreeHost(h_results);
         for (auto e : ev_pool) cudaEventDestroy(e);
@@ -522,6 +526,34 @@ struct Engine {
                        std::vector<uint64_t> &counts);
     int geo_filter_universes(const b200_query_batch *b, GeoFiltered &out);
     int geo_filter_batch(uint32_t n, const uint8_t *kind, const double *args, uint64_t *out, uint64_t out_words, int32_t *status);
+    // facet distribution (facet.cu, engine_facet.cpp).  A slot is one (candidate bitmap on the device, field); its outputs sit at
+    // index `slot` of the device outputs, which facet_results copies back and decodes into the caller's b200_results::facet_* arrays.
+    struct FacetJob {
+        const unsigned long long *cand;
+        uint16_t fid;
+        uint32_t slot;
+    };
+    struct FacetOut {
+        uint32_t *ord = nullptr, *doc = nullptr, *sum = nullptr;
+        unsigned long long *cnt = nullptr;
+        size_t n_slots = 0;
+        uint32_t cap = 0;
+    };
+    DevBuf<uint8_t> d_facet_scratch, d_facet_out;
+    DevBuf<FacetSlot> d_facet_slots;
+    DevBuf<unsigned long long> d_facet_cand;
+    size_t facet_slot_bytes(uint16_t fid) const;  // scratch of one slot
+    // the scratch and descriptors for `jobs`, processed in chunks of at most `budget` bytes of scratch (at least one slot)
+    int reserve_facet_scratch(const std::vector<uint16_t> &fids, size_t budget, DevBuf<uint8_t> &scratch, DevBuf<FacetSlot> &slots);
+    int reserve_facet_out(size_t n_slots, uint32_t cap, FacetOut &out);  // B200_ERR_CAPACITY when it does not fit
+    // enqueue the kernels of `jobs` on the lane's stream (ln), or on the handle's stream (ln == nullptr)
+    int facet_enqueue(Lane *ln, const std::vector<FacetJob> &jobs, const FacetOut &out, uint32_t max_values, DevBuf<uint8_t> &scratch,
+                      DevBuf<FacetSlot> &slots);
+    // after the kernels: the caller's outputs of slots [0, n_slots) (fid[k]); a slot needing more than out.cap entries gets its
+    // message in err[k] (empty otherwise) and empty outputs
+    int facet_results(const FacetOut &out, const uint16_t *fid, const b200_results &dst, std::vector<std::string> &err);
+    int facet_distribution_batch(uint32_t n, const uint64_t *const *candidates, uint64_t n_words, const uint32_t *begin, const uint16_t *fid,
+                                 const uint8_t *order, uint32_t max_values, uint32_t cap, const b200_results &dst, int32_t *status);
     ~Engine();
 };
 

@@ -18,16 +18,7 @@ namespace b200 {
 
 namespace {
 
-// f64 as Rust's Display writes it: the shortest digits that read back to the same value, never an exponent (a subnormal needs
-// some 1075 decimals, a value near DBL_MAX 309 integer digits)
-std::string rust_f64(double v) {
-    char buf[1500];
-    for (int p = 0; p <= 1100; p++) {
-        snprintf(buf, sizeof buf, "%.*f", p, v);
-        if (strtod(buf, nullptr) == v) break;
-    }
-    return buf;
-}
+std::string rust_f64(double v) { return rust_f64_display(v); }
 
 const char *const NON_FINITE = "Non finite floats are not supported";
 // FilterError::AttributeNotFilterable (filter/mod.rs:82-98) goes on with the index's filterable patterns, which the library does not

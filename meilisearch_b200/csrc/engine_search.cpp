@@ -1776,6 +1776,9 @@ struct KeywordBatch {
     const bool use_tree;
     // rule_start: the buckets of its single activation are collected here instead of being sorted further
     std::vector<RuleBucket> *rule_buckets = nullptr;
+    // facets (b200_query_batch::facet_*): computed from each query's candidates where schedule() hands them over
+    bool facets = false, facet_outputs = false;  // facet_outputs: facet_fid and every facet_* output are there
+    Engine::FacetOut fout;
     unsigned n_drivers = 1, lanes_per_driver = 1, n_lanes = 1;
     std::vector<std::vector<std::unique_ptr<Pending>>> lane_acts;  // per lane: the activations of its step in flight
     bool use_rowtab = false;
@@ -1846,6 +1849,53 @@ struct KeywordBatch {
                 q.done = true;
             }
         }
+    }
+    // ---- facets: the queries that cannot have them fail alone; the others' slots get device outputs, and every lane room for the
+    // counts of its queries' slots (in chunks of at most 64 MB when they are many)
+    void check_facets() {
+        facets = b->facet_begin != nullptr;
+        if (!facets) return;
+        const bool outputs = facet_outputs = b->facet_fid && r->facet_n_num && r->facet_n_str && r->facet_key && r->facet_count && r->facet_docid && r->facet_has_stats &&
+                             r->facet_min && r->facet_max;
+        for (uint32_t i = 0; i < NQ; i++) {
+            QState &q = *qs[i];
+            const uint32_t k0 = b->facet_begin[i], k1 = b->facet_begin[i + 1];
+            if (q.done || k1 <= k0) continue;
+            const char *why = nullptr;
+            int code = B200_ERR_UNSUPPORTED;
+            if (b->mode != 0)
+                why = "facets in a semantic or hybrid search (use b200_facet_distribution_batch over its candidates)";
+            else if (has_thr)
+                why = "facets together with a ranking-score threshold";
+            else if (!outputs)
+                code = B200_ERR_INVALID, why = "facet_begin without facet_fid or without the facet_* outputs";
+            else
+                for (uint32_t k = k0; k < k1 && b->facet_order && !why; k++)
+                    if (b->facet_order[k] == 1)
+                        why = "facet order by count (sortFacetValuesBy: count) is not built";
+                    else if (b->facet_order[k] > 1)
+                        code = B200_ERR_INVALID, why = "facet_order is not 0 (alpha) or 1 (count)";
+            if (why) {
+                q.status = code;
+                q.error = why;
+                q.done = true;
+            }
+        }
+    }
+    int setup_facets() {
+        if (!facets) return B200_OK;
+        const uint32_t n_slots = b->facet_begin[NQ];
+        int rc = eng.reserve_facet_out(n_slots, b->facet_cap, fout);
+        if (rc != B200_OK) return rc;
+        CU(cudaMemsetAsync(fout.sum, 0, (size_t)n_slots * 16, eng.stream), "zero facet outputs");
+        for (unsigned l = 0; l < n_lanes; l++) {
+            std::vector<uint16_t> fids;
+            for (uint32_t i : lanes[l].members)
+                if (!qs[i]->done)
+                    for (uint32_t k = b->facet_begin[i]; k < b->facet_begin[i + 1]; k++) fids.push_back(b->facet_fid[k]);
+            if ((rc = eng.reserve_facet_scratch(fids, (size_t)64 << 20, lanes[l].d_facet, lanes[l].d_facet_slots)) != B200_OK) return rc;
+        }
+        return B200_OK;
     }
     // ---- filtered universes (search/new/mod.rs:719): every distinct bitmap is intersected with documents_ids and uploaded once
     int stage_universes() {
@@ -2551,15 +2601,27 @@ struct KeywordBatch {
             for (auto &pd : q.pendings) cand_q.push_back(Cand{i, pd.get()});
             if (!q.emits.empty()) s.emit_q.push_back(i);
         }
-        if (r->candidates)
-            for (auto i : ln.members) {  // SearchResult::candidates, copied before any block freed above can be written again
+        if (r->candidates || facets) {
+            // SearchResult::candidates, copied and counted for the facets before any block freed above can be written again
+            std::vector<Engine::FacetJob> fjobs;
+            for (auto i : ln.members) {
                 QState &q = *qs[i];
                 if (!q.cand_src) continue;
-                CU(cudaMemcpyAsync(r->candidates + (size_t)i * r->candidates_words, q.cand_src, (size_t)hix.n_words64 * 8, cudaMemcpyDeviceToHost, ln.stream),
-                   "D2H candidates");
-                ln.lst.d2h_bytes += (size_t)hix.n_words64 * 8;
+                if (r->candidates) {
+                    CU(cudaMemcpyAsync(r->candidates + (size_t)i * r->candidates_words, q.cand_src, (size_t)hix.n_words64 * 8, cudaMemcpyDeviceToHost,
+                                       ln.stream),
+                       "D2H candidates");
+                    ln.lst.d2h_bytes += (size_t)hix.n_words64 * 8;
+                }
+                if (facets && q.status == 0)
+                    for (uint32_t k = b->facet_begin[i]; k < b->facet_begin[i + 1]; k++) fjobs.push_back(Engine::FacetJob{q.cand_src, b->facet_fid[k], k});
                 q.cand_src = nullptr;
             }
+            if (!fjobs.empty()) {
+                const int rc = eng.facet_enqueue(&ln, fjobs, fout, b->facet_max_values, ln.d_facet, ln.d_facet_slots);
+                if (rc != B200_OK) return rc;
+            }
+        }
         // longest first: the parallel-for over these queries ends when its slowest query does, and host time per query grows
         // with the size of its query graph
         std::stable_sort(cand_q.begin(), cand_q.end(), [&](const Cand &x, const Cand &y) { return x.pd->L->graph.nodes.size() > y.pd->L->graph.nodes.size(); });
@@ -3125,6 +3187,11 @@ struct KeywordBatch {
     }
     // fold the lanes' statistics (host phases of different lanes overlap in time); returns the first lane's error
     int fold_lane_stats() {
+        if (facets)  // facet kernels enqueued by a lane's last schedule() run after its last step: their timers are still open
+            for (unsigned l = 0; l < n_lanes; l++) {
+                CU(cudaStreamSynchronize(lanes[l].stream), "sync facets");
+                lanes[l].resolve_timers(lanes[l].lst);
+            }
         for (unsigned l = 0; l < n_lanes; l++) {
             const b200_stats &x = lanes[l].lst;
             stats.kernel_launches += x.kernel_launches;
@@ -3149,7 +3216,7 @@ struct KeywordBatch {
         }
         for (unsigned l = 0; l < n_lanes; l++)
             if (lanes[l].rc < 0) return lanes[l].rc;
-        if (r->candidates)
+        if (r->candidates || facets)
             for (unsigned l = 0; l < n_lanes; l++) CU(cudaStreamSynchronize(lanes[l].stream), "sync candidates");
         return B200_OK;
     }
@@ -3536,6 +3603,21 @@ struct KeywordBatch {
         stats.d2h_bytes += out_ids.size() * 4;
         stats.h2d_bytes += (size_t)b->lemma_off[b->token_begin[NQ]] + (size_t)b->token_begin[NQ] * 5 + (size_t)NQ * 4;
         CU(cudaStreamSynchronize(eng.stream), "sync");
+        if (facets && facet_outputs) {
+            std::vector<std::string> err;
+            const int rc = eng.facet_results(fout, b->facet_fid, *r, err);
+            if (rc != B200_OK) return rc;
+            for (uint32_t i = 0; i < NQ; i++) {
+                QState &q = *qs[i];
+                for (uint32_t k = b->facet_begin[i]; k < b->facet_begin[i + 1]; k++) {
+                    if (q.status == 0 && !err[k].empty()) {  // this slot needs more than facet_cap entries: the query fails alone
+                        q.status = B200_ERR_CAPACITY;
+                        q.error = err[k];
+                    }
+                    if (q.status != 0) r->facet_n_num[k] = r->facet_n_str[k] = r->facet_has_stats[k] = 0;
+                }
+            }
+        }
         for (uint32_t i = 0; i < NQ; i++) {
             QState &q = *qs[i];
             if (r->status) r->status[i] = q.status;
@@ -3707,8 +3789,10 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
     KeywordBatch kb(*this, b, r, offset, limit, scoring);
     kb.parse();
     kb.resolve_sort_rules();
+    kb.check_facets();
     int rc = kb.stage_universes();
     if (rc == B200_OK) rc = kb.setup_lanes();
+    if (rc == B200_OK) rc = kb.setup_facets();
     if (rc == B200_OK) rc = kb.drive_waves();
     if (rc == B200_OK) rc = kb.finish_batch();
     return rc;

@@ -89,8 +89,12 @@ Engine::~Engine() {
                     (void *)dix.emb, (void *)dix.emb_inv_norm, (void *)dix.emb_docids, (void *)arena, (void *)scratch})
         if (p) cudaFree(p);
     for (auto &kv : hix.sort_fields)
-        for (auto p : kv.second.d_key)
+        for (auto p : {kv.second.d_key[0], kv.second.d_key[1], kv.second.d_doc_off, kv.second.d_doc_ord, kv.second.d_disp})
             if (p) cudaFree(p);
+    d_facet_scratch.release();
+    d_facet_slots.release();
+    d_facet_out.release();
+    d_facet_cand.release();
     if (d_geo_pts) cudaFree(d_geo_pts);
     if (d_geo_ub) cudaFree(d_geo_ub);
     d_geo_count.release();
@@ -181,6 +185,18 @@ int Engine::stage_finish() {
             stats.hbm_bytes_staged += k.size() * 4;
             std::vector<uint32_t>().swap(k);
         }
+    // facet distribution: per faceted field its document-major ordinals and the Display order of its numbers
+    for (auto &kv : hix.sort_fields) {
+        SortField &f = kv.second;
+        auto src = [](const std::vector<uint32_t> &v) { return v.empty() ? nullptr : v.data(); };  // upload() allocates one element for none
+        CU(upload(&f.d_doc_off, src(f.doc_off), f.doc_off.size()), "upload facet ordinals");
+        CU(upload(&f.d_doc_ord, src(f.doc_ord), f.doc_ord.size()), "upload facet ordinals");
+        CU(upload(&f.d_disp, src(f.disp), f.disp.size()), "upload facet display order");
+        stats.hbm_bytes_staged += (f.doc_off.size() + f.doc_ord.size() + f.disp.size()) * 4;
+        std::vector<uint32_t>().swap(f.doc_off);
+        std::vector<uint32_t>().swap(f.doc_ord);
+        std::vector<uint32_t>().swap(f.disp);
+    }
     // GeoSort points: lat_lng_to_xyz (lib.rs:397-404) and cos(lat) with the host's libm, as the reference computes them
     {
         GeoField &g = hix.geo;

@@ -5,6 +5,8 @@
 #include "host_index.h"
 
 #include <algorithm>
+#include <charconv>
+#include <cstdlib>
 #include <stdexcept>
 #include <thread>
 
@@ -371,6 +373,72 @@ void build_sort_fields(const RawDb &f64_db, const RawDb &string_db, HostIndex &i
     };
     fold(nums, true);
     fold(strs, false);
+    // facet distribution: each number's f64 (the bound's last 8 bytes, big-endian), the number ordinals in Display-string order, and
+    // the document-major ordinals.  Filling the table value by value in ascending ordinal order leaves each document's run sorted.
+    for (uint64_t i = 0, l0 = 0; i < f64_db.n; i++) {
+        const uint8_t *k = f64_db.keys.data() + f64_db.koff[i];
+        if (k[2] != 0) continue;
+        uint64_t bits = 0;
+        for (int b = 0; b < 8; b++) bits = bits << 8 | k[11 + b];
+        double v;
+        memcpy(&v, &bits, 8);
+        ix.sort_fields[nums[l0++].fid].num_val.push_back(v);
+    }
+    for (auto &kv : ix.sort_fields) {
+        SortField &f = kv.second;
+        std::vector<std::string> shown(f.n_num);
+        for (uint32_t o = 0; o < f.n_num; o++) shown[o] = rust_f64_display(f.num_val[o]);
+        f.disp.resize(f.n_num);
+        for (uint32_t o = 0; o < f.n_num; o++) f.disp[o] = o;
+        std::sort(f.disp.begin(), f.disp.end(), [&](uint32_t a, uint32_t b) { return shown[a] < shown[b]; });
+        f.doc_off.assign(ix.n_docs + 1, 0);
+    }
+    auto each_value = [&](auto fn) {
+        seen.clear();
+        for (auto &x : nums) fn(ix.sort_fields[x.fid], seen[x.fid]++, x);
+        seen.clear();
+        for (auto &x : strs) {
+            SortField &f = ix.sort_fields[x.fid];
+            fn(f, f.n_num + seen[x.fid]++, x);
+        }
+    };
+    each_value([&](SortField &f, uint32_t, const Val &x) {
+        for (uint32_t d : x.docs)
+            if (d < ix.n_docs) f.doc_off[d + 1]++;
+    });
+    for (auto &kv : ix.sort_fields) {
+        SortField &f = kv.second;
+        for (uint32_t d = 0; d < ix.n_docs; d++) f.doc_off[d + 1] += f.doc_off[d];
+        f.doc_ord.resize(f.doc_off[ix.n_docs]);
+    }
+    std::map<uint16_t, std::vector<uint32_t>> fill;
+    each_value([&](SortField &f, uint32_t o, const Val &x) {
+        std::vector<uint32_t> &at = fill[x.fid];
+        if (at.empty()) at.assign(f.doc_off.begin(), f.doc_off.end() - 1);
+        for (uint32_t d : x.docs)
+            if (d < ix.n_docs) f.doc_ord[at[d]++] = o;
+    });
+}
+
+std::string rust_f64_display(double v) {
+    if (std::isnan(v)) return "NaN";
+    if (std::isinf(v)) return v > 0 ? "inf" : "-inf";
+    // to_chars in scientific notation gives the shortest round-trip digits d[.ddd]e±x; fixed notation would print the exact binary
+    // expansion of a large value ("99999999999999991611392" for 1e23) where Rust pads the shortest digits with zeros
+    char buf[64];
+    const auto res = std::to_chars(buf, buf + sizeof buf, v, std::chars_format::scientific);
+    std::string s(buf, res.ptr), sign;
+    if (s[0] == '-') {
+        sign = "-";
+        s.erase(0, 1);
+    }
+    const size_t e = s.find('e');
+    const int point = 1 + atoi(s.c_str() + e + 1);  // decimal point position after the first digit, shifted by the exponent
+    std::string digits = s.substr(0, e);
+    if (digits.size() > 1) digits.erase(1, 1);  // the '.'
+    if (point <= 0) return sign + "0." + std::string((size_t)-point, '0') + digits;
+    if ((size_t)point >= digits.size()) return sign + digits + std::string((size_t)point - digits.size(), '0');
+    return sign + digits.substr(0, (size_t)point) + "." + digits.substr((size_t)point);
 }
 
 void build_geo_field(const RawDb &f64_db, const RawDb &string_db, HostIndex &ix) {

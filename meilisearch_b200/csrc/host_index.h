@@ -59,6 +59,11 @@ struct SortField {
     std::vector<uint32_t> num_key, str_key;  // value i -> position among the staged level-0 keys of its database
     std::vector<uint32_t> key[2];            // [0] ascending, [1] descending: u32[n_docs], released after upload
     uint32_t *d_key[2] = {nullptr, nullptr}; // the same in HBM
+    // Facet distribution (facet.cu): every document's ascending ordinals, sorted (CSR: doc_off u32[n_docs + 1] into doc_ord), the
+    // number ordinals in the order of their f64 Display strings (disp), released after upload; the f64 of each number ordinal
+    std::vector<uint32_t> doc_off, doc_ord, disp;
+    uint32_t *d_doc_off = nullptr, *d_doc_ord = nullptr, *d_disp = nullptr;
+    std::vector<double> num_val;
     uint32_t n_values() const { return n_num + n_str; }
     // ordinal of direction `asc` -> (is_string, position among the level-0 keys of its database)
     void decode(bool asc, uint32_t o, bool &is_string, uint32_t &key_index) const {
@@ -205,6 +210,8 @@ void build_host_index(const std::vector<uint8_t> &dict_bytes, const std::vector<
 // Decode the level-0 entries of facet_id_f64_docids / facet_id_string_docids into out.sort_fields (after build_host_index: needs
 // n_docs).  Throws std::runtime_error on a malformed key or value.
 void build_sort_fields(const RawDb &f64_db, const RawDb &string_db, HostIndex &out);
+// Rust's `impl Display for f64`: the shortest digits that read back as the same value, never an exponent ("-0" for -0.0)
+std::string rust_f64_display(double v);
 // Read every document's point into out.geo (after build_host_index; out.geo.lat_fid / lng_fid set, or nothing to do).  Throws
 // std::runtime_error for a document with one coordinate only or a string coordinate that does not parse as f64.
 void build_geo_field(const RawDb &f64_db, const RawDb &string_db, HostIndex &out);

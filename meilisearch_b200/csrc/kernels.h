@@ -38,6 +38,9 @@ cudaError_t launch_geo_first_fail(cudaStream_t s, const unsigned long long *geo,
                                   const uint32_t *radius, uint32_t n_radius, GeoFirst *first);
 cudaError_t launch_geo_filter(cudaStream_t s, const unsigned long long *geo, const GeoPoint *pts, uint32_t n_words, const GeoClause *clauses,
                               const GeoFirst *first, const uint32_t *slot_clauses, const GeoSlot *slots, uint32_t n_slots);
+// facet.cu: counts of every slot's values over its candidates (FacetSlot scratch zero at launch), then one CTA per slot selects the
+// entries the reference's facet_values returns
+cudaError_t launch_facet(cudaStream_t s, const FacetSlot *slots, uint32_t n_slots, uint32_t n_words, uint32_t n_docs);
 cudaError_t launch_vec_dist(cudaStream_t s, int n_ctas, int qt, const void *mat_fp16, const float *inv_norm, const uint32_t *docids,
                             uint64_t n_rows, uint32_t d, const float *queries, const float *q_inv_norm, const unsigned long long *cand,
                             uint64_t n_cand_words, float *dist);
