@@ -23,6 +23,13 @@ def normalize_facet(s: str) -> str:
     return unicodedata.normalize("NFKD", s.strip()).lower()
 
 
+def hyper_normalize(s: str) -> str:
+    """The facet-search key of an already normalize_facet'd value: NFKD, combining marks dropped, lower-cased.  This only
+    approximates charabia's lossy normaliser, which indexing uses (update/new/facet_search_builder.rs); the library never
+    recomputes it and reads whatever facet_id_normalized_string_strings holds."""
+    return "".join(c for c in unicodedata.normalize("NFKD", s) if not unicodedata.combining(c)).lower()
+
+
 def ordered_f64(f: float) -> bytes:
     """OrderedF64Codec: globally ordered bytes (facet/value_encoding.rs f64_into_bytes), then the f64 big-endian"""
     f = float(f)
@@ -192,6 +199,36 @@ class FacetImage:
         self.f64_db = _db(self._entries(self.numbers, lambda v: ordered_f64(v)))
         self.string_db = _db(self._entries(self.strings, lambda v: v.encode()))
         return self.f64_db, self.string_db
+
+    def build_search(self):
+        """-> (facet_id_normalized_string_strings, field_id_docid_facet_strings) as DbImage, keys in LMDB order: per string field
+        every hyper-normalised string with the JSON set of the level-0 keys it stands for, and every (fid, docid, normalised key)
+        with its original string.  Also kept as self.norm_db / self.orig_db, which Index.stage stages when present."""
+        import json
+
+        norm = []
+        for fid, vals in self.strings.items():
+            groups = {}
+            for v in vals:
+                groups.setdefault(hyper_normalize(v), []).append(v)
+            for h, keys in groups.items():
+                keys = sorted(keys, key=lambda s: s.encode())  # BTreeSet<String> order
+                norm.append((struct.pack(">H", fid) + h.encode(), json.dumps(keys, ensure_ascii=False, separators=(",", ":")).encode()))
+        norm.sort(key=lambda e: e[0])
+        orig = sorted((struct.pack(">HI", f, d) + v.encode(), o.encode()) for (f, d, v), o in self.originals.items())
+        self.norm_db, self.orig_db = _db(norm), _db(orig)
+        return self.norm_db, self.orig_db
+
+    def add_synthetic_search(self, n_docs, n_values=100_000, seed=0x5EA7):
+        """seeded `model`: a high-cardinality string field (n_values distinct values, one per document, the rest drawn uniformly) of
+        lower-case letter-and-digit words, for facet search at scale"""
+        rng = np.random.default_rng(seed)
+        letters = np.array(list("abcdefghijklmnopqrstuvwxyz"))
+        lens = rng.integers(4, 11, n_values)
+        words = np.array(["".join(rng.choice(letters, n)) + str(i) for i, n in enumerate(lens)])
+        pick = np.concatenate([np.arange(min(n_values, n_docs)), rng.integers(0, n_values, max(0, n_docs - n_values))])
+        self._bulk("model", np.arange(n_docs, dtype=np.uint32), words[pick[:n_docs]], numbers=False)
+        return self
 
     @staticmethod
     def _entries(tab, enc):

@@ -55,7 +55,17 @@ enum b200_db {
      * u8 size | CBO bytes (heed_codec/facet/mod.rs).  Only level-0 entries are read; higher levels are accepted and ignored. */
     B200_DB_FACET_ID_F64_DOCIDS = 10,
     B200_DB_FACET_ID_STRING_DOCIDS = 11,
-    B200_DB_COUNT = 12
+    /* facet databases read by facet search (search/facet/search.rs:119-265).  facet_id_normalized_string_strings: key u16 BE fid |
+     * hyper-normalised string, value the serde_json bytes of the BTreeSet<String> of level-0 keys of facet_id_string_docids it
+     * stands for (index.rs facet_id_normalized_string_strings).  A field's facet-string FST (facet_id_string_fst) holds exactly
+     * the keys of its entries here: indexing registers every key it writes or deletes in this database with the FST merger
+     * (update/new/facet_search_builder.rs:148-213), so a shim may stage the keys from either source.  A value that is not a JSON
+     * array of strings makes b200_stage_finish fail with B200_ERR_INVALID.
+     * field_id_docid_facet_strings: key u16 BE fid | u32 BE docid | normalised string, value the original string
+     * (heed_codec/facet/field_doc_id_facet_codec.rs, index.rs:181-188). */
+    B200_DB_FACET_ID_NORMALIZED_STRING_STRINGS = 12,
+    B200_DB_FIELD_ID_DOCID_FACET_STRINGS = 13,
+    B200_DB_COUNT = 14
 };
 /* Replaces Index::words_fst (index.rs:1238): the FST enumerated once on the host into its sorted word list. */
 int b200_stage_dictionary(b200_index *, const uint8_t *word_bytes, const uint64_t *word_offsets, uint64_t n_words);
@@ -251,6 +261,23 @@ typedef struct {
     const uint8_t *facet_order;
     uint32_t facet_max_values;
     uint32_t facet_cap;
+    /* Facet search over each query's candidates (perform_facet_search, crates/meilisearch/src/search/mod.rs:2514-2574, with
+     * execute_for_candidates, search/mod.rs:254-278), as b200_facet_search_batch answers it: query i searches field
+     * facet_search_fid[i] (0xFFFF: no facet search for that query; facet_search_fid NULL: none anywhere) with facet_query_kind[i]
+     * (0 None, 1 Some), the query bytes facet_query_bytes[facet_query_off[i] .. facet_query_off[i + 1]) and facet_search_flags[i]
+     * (bit 0 order by count, bit 1 the field is not an exact attribute), keeping at most facet_search_max hits, which is also the
+     * stride of the b200_results::fs_* outputs.  The candidates are, in mode 0, exactly the bitmap `candidates` holds
+     * (SearchResult::candidates, degraded results included), copied on the device where the search hands it over, and in modes 1
+     * and 2 the query's filtered universe (documents_ids AND universes[i] AND its geo clauses); they never cross PCIe.  Per query: a
+     * facet search with a ranking-score threshold is B200_ERR_UNSUPPORTED; facet_search_fid without facet_query_kind,
+     * facet_search_flags or the fs_* outputs (or without facet_query_off / facet_query_bytes when a kind is 1) is B200_ERR_INVALID;
+     * the errors of b200_facet_search_batch apply to the query alone (its search results are then dropped as well). */
+    const uint16_t *facet_search_fid;
+    const uint8_t *facet_query_kind;
+    const uint32_t *facet_query_off;
+    const char *facet_query_bytes;
+    const uint8_t *facet_search_flags;
+    uint32_t facet_search_max;
 } b200_query_batch;
 #define B200_MAX_SCORES 12
 /* score kinds: ScoreDetails variants (score_details.rs:9-32) */
@@ -301,6 +328,13 @@ typedef struct {                  /* SearchResult (search/mod.rs:526-535), flatt
     uint8_t *facet_has_stats;
     double *facet_min;
     double *facet_max;
+    /* Facet search of query i (b200_query_batch::facet_search_*): fs_n[i] hits at [i * facet_search_max, ..), each as in
+     * b200_facet_search_batch (key, count, docid, fallback). */
+    uint32_t *fs_n;
+    uint32_t *fs_key;
+    uint64_t *fs_count;
+    uint32_t *fs_docid;
+    uint8_t *fs_fallback;
 } b200_results;
 int b200_search_batch(b200_index *, const b200_query_batch *, b200_results *);
 
@@ -320,6 +354,36 @@ int b200_facet_distribution_batch(b200_index *, uint32_t n, const uint64_t *cons
                                   const uint16_t *facet_fid, const uint8_t *facet_order, uint32_t max_values, uint32_t cap, uint32_t *n_num,
                                   uint32_t *n_str, uint32_t *key, uint64_t *count, uint32_t *docid, uint8_t *has_stats, double *min,
                                   double *max, int32_t *status);
+
+/* Replaces SearchForFacetValues::execute after its facet-searchable check and field resolution (search/facet/search.rs:74-265), as
+ * called by perform_facet_search (crates/meilisearch/src/search/mod.rs:2514-2574) with the candidates of execute_for_candidates
+ * (search/mod.rs:254-278), for callers that hold the candidates themselves.  Request i searches field fid[i] (its id in the facet
+ * databases; 0xFFFF or a field without facet_id_normalized_string_strings entries: no FST, an empty answer) over the host bitmap
+ * candidates[i] (dense little-endian u64 words, n_words >= ceil((max docid + 1) / 64), NULL entry = documents_ids; equal pointers
+ * are uploaded once).
+ *   kind[i] 0 (query None): every level-0 key of facet_id_string_docids for the field, in key order (:224-240).
+ *   kind[i] 1 (Some(q)): q = query_bytes[off[i] .. off[i + 1]) (off has n + 1 entries), already normalize_facet_string'd by the
+ *     caller.  With typos allowed (flags bit 1 set, meaning the field is not an exact attribute, and the staged authorize_typos):
+ *     when q is in the staged exact_words, the one string q if the FST holds it; otherwise the FST strings accepted by
+ *     build_dfa(q, k, prefix = true) (search/mod.rs:565-577): the minimum restricted Damerau-Levenshtein (OSA) distance between q and a
+ *     prefix of the string, over Unicode scalar values, is at most k = 0 / 1 / 2 as q's byte length is below min_word_len_one_typo
+ *     / below min_word_len_two_typos / neither, with no first-letter rule.  Without typos: the FST strings that start with q.
+ *     Matches are walked in byte order; each one's level-0 keys in its JSON set order, stopping at a key that facet_id_string_docids
+ *     lacks (:242-289).  q longer than B200_FACET_QUERY_MAX Unicode scalar values is B200_ERR_UNSUPPORTED for that request.
+ * Every walked key whose docids meet the candidates is a hit: count = |docids AND candidates|.  flags bit 0 clear: the first `max`
+ * hits (OrderBy::Lexicographic); set: OrderBy::Count, the BinaryHeap<Reverse<FacetValueHit>> replay of ValuesCollection::insert
+ * (:292-353) ordered by (count, value bytes), output in descending order.  A hit's value is the original string at (fid, docid,
+ * key) in field_id_docid_facet_strings, where docid is the smallest of all the key's docids, or, without that entry, q (kind 1) or
+ * the key (kind 0).
+ * Outputs, stride `cap` per request: n_out[i] hits; key[i * cap + j] the hit's position among the staged level-0 keys of
+ * facet_id_string_docids (as B200_S_SORT's score_rank), count, docid (the smallest docid of the key) and fallback (1: no original,
+ * the value is q or the key).  status[i]: 0; B200_ERR_UNSUPPORTED (query too long); B200_ERR_INVALID (kind > 1, or off not
+ * ascending); B200_ERR_CAPACITY (min(max, hits) > cap), for that request alone, with n_out[i] = 0.  max = 0 answers nothing. */
+#define B200_FACET_QUERY_MAX 64
+int b200_facet_search_batch(b200_index *, uint32_t n, const uint64_t *const *candidates, uint64_t n_words, const uint16_t *fid,
+                            const uint8_t *kind, const uint32_t *off, const char *query_bytes, const uint8_t *flags, uint32_t max,
+                            uint32_t cap, uint32_t *n_out, uint32_t *key, uint64_t *count, uint32_t *docid, uint8_t *fallback,
+                            int32_t *status);
 
 /* ---- S1: the RankingRule seam ---------------------------------------------------------- */
 /* Replaces `dyn RankingRule` as driven by bucket_sort (crates/milli/src/search/new/ranking_rules.rs:26-83, bucket_sort.rs:123,266,323)
@@ -350,7 +414,7 @@ void b200_rule_end(b200_rule *);
 /* kernel classes for the per-kernel accounting below */
 enum b200_kernel { B200_K_LEV = 0, B200_K_COMPACT = 1, B200_K_PAIR_PROBE = 2, B200_K_SCATTER = 3, B200_K_EVAL_PATHS = 4, B200_K_EMIT = 5,
                    B200_K_VEC_DIST = 6, B200_K_TOPK = 7, B200_K_VEC_GEMM = 8, B200_K_VEC_MERGE = 9, B200_K_SORT = 10, B200_K_GEO = 11,
-                   B200_K_GEO_FILTER = 12, B200_K_FACET = 13, B200_K_COUNT = 14 };
+                   B200_K_GEO_FILTER = 12, B200_K_FACET = 13, B200_K_FACET_SEARCH = 14, B200_K_COUNT = 15 };
 typedef struct {
     uint64_t kernel_launches;     /* kernels launched by the library since the last reset */
     uint64_t device_steps;        /* host<->device round trips since the last reset */

@@ -25,6 +25,7 @@ TMS = {"last": 0, "all": 1, "frequency": 2}
 SCORE_KINDS = ["words", "typo", "proximity", "fid", "position", "exactAttribute", "exactWords", "vector", "skipped", "sort", "geo"]
 GEO_STRATEGIES = {"dynamic": 0, "iterative": 1, "rtree": 2}  # GeoSortStrategy::Dynamic / AlwaysIterative / AlwaysRtree
 DB_FACET_F64, DB_FACET_STRING = 10, 11
+DB_FACET_NORMALIZED, DB_FACET_ORIGINALS = 12, 13  # facet_id_normalized_string_strings, field_id_docid_facet_strings
 NO_FIELD = 0xFFFF  # a sort field absent from the fields map
 ERRORS = {-1: "NO_DEVICE", -2: "CUDA", -3: "INVALID", -4: "UNSUPPORTED", -5: "CAPACITY", -6: "STATE"}
 
@@ -51,7 +52,9 @@ class _Batch(C.Structure):
                 ("sort_geo", C.c_void_p), ("sort_geo_point", C.c_void_p), ("geo_strategy", C.c_int32), ("geo_cache_size", C.c_uint32),
                 ("geo_max_bucket_size", C.c_uint64), ("geo_filter_begin", C.c_void_p), ("geo_filter_kind", C.c_void_p),
                 ("geo_filter_not", C.c_void_p), ("geo_filter_args", C.c_void_p), ("facet_begin", C.c_void_p), ("facet_fid", C.c_void_p),
-                ("facet_order", C.c_void_p), ("facet_max_values", C.c_uint32), ("facet_cap", C.c_uint32)]
+                ("facet_order", C.c_void_p), ("facet_max_values", C.c_uint32), ("facet_cap", C.c_uint32), ("facet_search_fid", C.c_void_p),
+                ("facet_query_kind", C.c_void_p), ("facet_query_off", C.c_void_p), ("facet_query_bytes", C.c_void_p),
+                ("facet_search_flags", C.c_void_p), ("facet_search_max", C.c_uint32)]
 
 
 class _Results(C.Structure):
@@ -59,18 +62,19 @@ class _Results(C.Structure):
                                           "n_candidates", "semantic_hits", "status", "degraded", "used_negative_operator", "candidates")] + \
                [("candidates_words", C.c_uint64)] + \
                [(n, C.c_void_p) for n in ("facet_n_num", "facet_n_str", "facet_key", "facet_count", "facet_docid", "facet_has_stats", "facet_min",
-                                          "facet_max")]
+                                          "facet_max")] + \
+               [(n, C.c_void_p) for n in ("fs_n", "fs_key", "fs_count", "fs_docid", "fs_fallback")]
 
 
 class _Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("device_steps", C.c_uint64), ("posting_bytes", C.c_uint64), ("matrix_bytes", C.c_uint64),
-                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 14),
-                ("kernel_count", C.c_uint64 * 14), ("kernel_bytes", C.c_uint64 * 14), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
+                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 15),
+                ("kernel_count", C.c_uint64 * 15), ("kernel_bytes", C.c_uint64 * 15), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
                 ("hbm_bytes_staged", C.c_uint64), ("deferred", C.c_uint64), ("arena_peak_bytes", C.c_uint64),
                 ("eval_class_launches", C.c_uint64 * 9), ("eval_class_tiles", C.c_uint64 * 9)]
 
 
-KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort", "geo", "geo_filter", "facet"]
+KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort", "geo", "geo_filter", "facet", "facet_search"]
 
 
 def build_library(force=False):
@@ -117,6 +121,8 @@ def load_library():
         l.b200_geo_filter_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
         l.b200_facet_distribution_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
                                                     C.c_uint32] + [C.c_void_p] * 9
+        l.b200_facet_search_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64] + [C.c_void_p] * 5 + [C.c_uint32, C.c_uint32] + \
+            [C.c_void_p] * 6
         l.b200_proximity_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
         l.b200_graph_from_tokens.argtypes = [C.c_void_p, C.POINTER(_Batch), C.POINTER(C.c_void_p)]
         l.b200_graph_free.argtypes = [C.c_void_p]
@@ -131,7 +137,7 @@ def load_library():
 
 SYMBOLS = ["b200_open", "b200_close", "b200_last_error", "b200_open_error", "b200_stage_dictionary", "b200_stage_db",
            "b200_stage_documents_ids", "b200_stage_settings", "b200_stage_synonyms", "b200_stage_geo_fields", "b200_stage_finish", "b200_stage_embeddings", "b200_stage_embeddings_f16", "b200_stage_distribution",
-           "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_geo_filter_batch", "b200_facet_distribution_batch", "b200_graph_from_tokens",
+           "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_geo_filter_batch", "b200_facet_distribution_batch", "b200_facet_search_batch", "b200_graph_from_tokens",
            "b200_graph_free", "b200_rule_start", "b200_rule_next", "b200_rule_end", "b200_get_stats", "b200_reset_stats"]
 
 
@@ -179,6 +185,7 @@ def _p(a):
 
 FACET_ORDERS = {"alpha": 0, "count": 1}  # OrderBy::Lexicographic / OrderBy::Count (sortFacetValuesBy)
 DEFAULT_VALUES_PER_FACET = 100  # facet_distribution.rs DEFAULT_VALUES_PER_FACET
+DEFAULT_MAX_FACET_SEARCH_VALUES = 100  # search/facet/search.rs DEFAULT_MAX_NUMBER_OF_VALUES_PER_FACET
 
 
 def rust_f64_display(x):
@@ -260,6 +267,13 @@ class SearchResult:
         self.used_negative_operator = np.zeros(n, np.uint8)
         self.candidates = None  # (n, words) uint64 when requested with Search.with_candidates()
         self._facets = None  # (index, per query its field names, begin, _FacetOutputs, max values) with Search.facets()
+        self._facet_search = None  # (index, per query (fid, query or None), outputs) with Search.facet_search()
+
+    def facet_hits(self, q):
+        """facetHits of query q's facet search: [(value, count), ...] in the reference's order"""
+        ix, per_q, (n_out, key, count, docid, fallback, mx) = self._facet_search
+        fid, query = per_q[q]
+        return ix._facet_hits(fid, query, key[q * mx:q * mx + int(n_out[q])], count[q * mx:], docid[q * mx:], fallback[q * mx:])
 
     def facet_distribution(self, q):
         """facetDistribution of query q: {field name: [(key, count), ...]} in the reference's order"""
@@ -335,6 +349,9 @@ class Index:
             for is_string, (dbid, db) in enumerate(((DB_FACET_F64, facets.f64_db), (DB_FACET_STRING, facets.string_db))):
                 self._ck(l.b200_stage_db(self._h, dbid, db.n_keys, _p(db.key_bytes), _p(db.key_offsets), _p(db.val_bytes), _p(db.val_offsets)))
                 self._level0[is_string] = [db.key(i) for i in range(db.n_keys) if db.key(i)[2] == 0]
+            for dbid, db in ((DB_FACET_NORMALIZED, getattr(facets, "norm_db", None)), (DB_FACET_ORIGINALS, getattr(facets, "orig_db", None))):
+                if db is not None:
+                    self._ck(l.b200_stage_db(self._h, dbid, db.n_keys, _p(db.key_bytes), _p(db.key_offsets), _p(db.val_bytes), _p(db.val_offsets)))
         self._n_docs = int(image.n_docs)
         self._ck(l.b200_stage_dictionary(self._h, _p(image.dict_bytes), _p(image.dict_offsets), image.n_words))
         for i, db in enumerate(image.dbs):
@@ -557,6 +574,47 @@ class Index:
             stats.append({name: out.stats(k) for name, k in zip(per[i], ks) if out.stats(k) is not None})
         return dists, stats, status[:n]
 
+    def facet_search(self, candidates, name, query=None, order="alpha", max_values=DEFAULT_MAX_FACET_SEARCH_VALUES, typos=True, cap=None):
+        """SearchForFacetValues::execute for candidate bitmaps the caller holds (b200_facet_search_batch): candidates: a list of
+        uint64 word arrays (None entries: documents_ids); name: the field; query: None, or the already normalised query, or one such
+        value per bitmap; typos: the field is not an exact attribute -> (per bitmap [(value, count), ...] in the reference's order,
+        statuses)"""
+        n = len(candidates)
+        qs = list(query) if isinstance(query, (list, tuple)) else [query] * n
+        fid = np.full(max(n, 1), self.field_id(name), np.uint16)
+        kind = np.asarray([0 if q is None else 1 for q in qs] or [0], np.uint8)
+        enc = [b"" if q is None else q.encode() for q in qs]
+        off = np.zeros(n + 1, np.uint32)
+        off[1:] = np.cumsum([len(b) for b in enc]) if n else []
+        qb = np.frombuffer(b"".join(enc) + b"\0", np.uint8).copy()
+        flags = np.full(max(n, 1), (FACET_ORDERS[order]) | (2 if typos else 0), np.uint8)
+        cap = max(1, max_values) if cap is None else cap
+        cache = {}
+        arrs = [None if c is None else cache.setdefault(id(c), np.ascontiguousarray(c, np.uint64)) for c in candidates]
+        ptrs = (C.c_void_p * max(n, 1))(*[None if a is None else a.ctypes.data for a in arrs])
+        words = next((len(a) for a in arrs if a is not None), (self._n_docs + 63) // 64)
+        n_out = np.zeros(max(n, 1), np.uint32)
+        key = np.zeros(max(n * cap, 1), np.uint32)
+        count = np.zeros(max(n * cap, 1), np.uint64)
+        docid = np.zeros(max(n * cap, 1), np.uint32)
+        fallback = np.zeros(max(n * cap, 1), np.uint8)
+        status = np.zeros(max(n, 1), np.int32)
+        self._ck(self._l.b200_facet_search_batch(self._h, n, C.cast(ptrs, C.c_void_p), words, _p(fid), _p(kind), _p(off), _p(qb), _p(flags),
+                                                 max_values, cap, _p(n_out), _p(key), _p(count), _p(docid), _p(fallback), _p(status)))
+        out = [self._facet_hits(int(fid[i]), qs[i], key[i * cap:i * cap + int(n_out[i])], count[i * cap:], docid[i * cap:], fallback[i * cap:])
+               for i in range(n)]
+        return out, status[:n]
+
+    def _facet_hits(self, fid, query, key, count, docid, fallback):
+        """FacetValueHit { value, count } of each returned hit: the original string of (fid, docid, level-0 key), or the query (the key
+        itself without a query) when fallback is set"""
+        hits = []
+        for e in range(len(key)):
+            k = self._level0[1][int(key[e])][3:].decode()
+            value = (query if query is not None else k) if fallback[e] else self.facet_original(fid, int(docid[e]), k)
+            hits.append((value, int(count[e])))
+        return hits
+
     def stats(self):
         s = _Stats()
         self._l.b200_get_stats(self._h, C.byref(s))
@@ -637,6 +695,7 @@ class Search:
         self._geo_strategy, self._geo_max_bucket = (0, 1000), 1000
         self._geo_filter = None
         self._facet_names, self._max_values, self._facet_order, self._facet_cap = None, DEFAULT_VALUES_PER_FACET, "alpha", None
+        self._fsearch = None
 
     def query(self, queries, stop_words=frozenset()):
         self._tokens = queries if isinstance(queries, TokenBatch) else TokenBatch([queries] if isinstance(queries, str) else list(queries), stop_words)
@@ -700,6 +759,13 @@ class Search:
         """geo leaves at the top of the filter, ANDed with the universe: ["_geoRadius(48.85, 2.35, 2000)", "NOT _geoBoundingBox([1, 2],
         [0, 1])"] for every query of the batch, or one such list per query (see parse_geo_filter)"""
         self._geo_filter = clauses
+        return self
+
+    def facet_search(self, name, query=None, order="alpha", max_values=DEFAULT_MAX_FACET_SEARCH_VALUES, typos=True):
+        """a facet search over each query's candidates (the facet-search route): field `name` (None: no facet search for that query),
+        the already normalised query (None or a string), sortFacetValuesBy, maxValuesPerFacet, and whether the field allows typos (it
+        is not an exact attribute).  name and query may be lists, one entry per query."""
+        self._fsearch = (name, query, order, max_values, typos)
         return self
 
     def facets(self, names):
@@ -805,6 +871,24 @@ class Search:
             (r.facet_n_num, r.facet_n_str, r.facet_key, r.facet_count, r.facet_docid, r.facet_has_stats, r.facet_min,
              r.facet_max) = out.pointers()
             res._facets = (ix, per_q, out.begin, out, self._max_values)
+        if self._fsearch is not None:
+            name, query, order, mx, typos = self._fsearch
+            names = list(name) if isinstance(name, (list, tuple)) else [name] * n
+            qs = list(query) if isinstance(query, (list, tuple)) else [query] * n
+            fid = np.asarray([NO_FIELD if nm is None else ix.field_id(nm) for nm in names] or [NO_FIELD], np.uint16)
+            kind = np.asarray([0 if q is None else 1 for q in qs] or [0], np.uint8)
+            enc = [b"" if q is None else q.encode() for q in qs]
+            off = np.zeros(n + 1, np.uint32)
+            off[1:] = np.cumsum([len(x) for x in enc]) if n else []
+            qb = np.frombuffer(b"".join(enc) + b"\0", np.uint8).copy()
+            flags = np.full(max(n, 1), FACET_ORDERS[order] | (2 if typos else 0), np.uint8)
+            outs = (np.zeros(max(n, 1), np.uint32), np.zeros(max(n * mx, 1), np.uint32), np.zeros(max(n * mx, 1), np.uint64),
+                    np.zeros(max(n * mx, 1), np.uint32), np.zeros(max(n * mx, 1), np.uint8))
+            keep += [fid, kind, off, qb, flags]
+            b.facet_search_fid, b.facet_query_kind, b.facet_query_off, b.facet_query_bytes = _p(fid), _p(kind), _p(off), _p(qb)
+            b.facet_search_flags, b.facet_search_max = _p(flags), mx
+            r.fs_n, r.fs_key, r.fs_count, r.fs_docid, r.fs_fallback = (_p(a) for a in outs)
+            res._facet_search = (ix, [(int(fid[q]), qs[q]) for q in range(n)], outs + (mx,))
         if self._want_candidates:
             words = (ix._n_docs + 63) // 64
             res.candidates = np.zeros((n, words), np.uint64)

@@ -306,6 +306,17 @@ int b200_facet_distribution_batch(b200_index *h, uint32_t n, const uint64_t *con
         return h->e.facet_distribution_batch(n, candidates, n_words, facet_begin, facet_fid, facet_order, max_values, cap, dst, status);
     });
 }
+int b200_facet_search_batch(b200_index *h, uint32_t n, const uint64_t *const *candidates, uint64_t n_words, const uint16_t *fid,
+                            const uint8_t *kind, const uint32_t *off, const char *query_bytes, const uint8_t *flags, uint32_t max,
+                            uint32_t cap, uint32_t *n_out, uint32_t *key, uint64_t *count, uint32_t *docid, uint8_t *fallback,
+                            int32_t *status) {
+    return guarded(h, [&]() -> int {
+        std::lock_guard<std::mutex> g(h->e.mu);
+        if (!h->e.staged) return h->e.fail(B200_ERR_STATE, "facet search before b200_stage_finish");
+        return h->e.facet_search_batch(n, candidates, n_words, fid, kind, off, query_bytes, flags, max, cap, n_out, key, count, docid,
+                                       fallback, status);
+    });
+}
 int b200_get_stats(b200_index *h, b200_stats *out) {
     std::lock_guard<std::mutex> g(h->e.mu);
     *out = h->e.stats;
@@ -516,7 +527,15 @@ int Engine::search_batch(const b200_query_batch *b, b200_results *r) {
 }
 
 int Engine::search_batch_filtered(const b200_query_batch *b, b200_results *r) {
-    if (b->mode == 0) return keyword_batch(b, r, b->offset, b->limit, b->scoring_strategy);
+    if (b->mode == 0) {
+        int rc = keyword_batch(b, r, b->offset, b->limit, b->scoring_strategy);
+        if (rc != B200_OK || !b->facet_search_fid) return rc;
+        // each query's candidates, copied on the device where the search handed them over (KeywordBatch::setup_facet_search)
+        std::vector<const unsigned long long *> dcand(b->n_queries, nullptr);
+        for (uint32_t q = 0; q < b->n_queries; q++)
+            if (q < fs_slot.size() && fs_slot[q] >= 0) dcand[q] = d_fs_qcand.p + (size_t)fs_slot[q] * hix.n_words64;
+        return search_facet_search(b, r, dcand);
+    }
     if (b->has_ranking_score_threshold || b->time_budget_ns || b->stop_after >= 0 || r->candidates)
         return fail(B200_ERR_UNSUPPORTED, "ranking-score threshold, deadlines and the candidates bitmap are implemented for keyword searches (mode 0) only");
     if (b->mode == 1) {
@@ -550,6 +569,11 @@ int Engine::search_batch_filtered(const b200_query_batch *b, b200_results *r) {
                 if (r->status) r->status[q] = code;
                 if (r->n_candidates) r->n_candidates[q] = 0;
             }
+        if (rc1 == B200_OK && b->facet_search_fid) {  // execute_for_candidates: the filtered universe (search/mod.rs:254-278)
+            std::vector<const unsigned long long *> dcand;
+            rc1 = filtered_universes(b, dcand);
+            if (rc1 == B200_OK) rc1 = search_facet_search(b, r, dcand);
+        }
         return rc1;
     }
     if (b->mode != 2) return fail(B200_ERR_INVALID, "unknown search mode");
@@ -678,6 +702,12 @@ int Engine::search_batch_filtered(const b200_query_batch *b, b200_results *r) {
         pool->run(NQ, merge_one);
     else
         for (uint32_t q = 0; q < NQ; q++) merge_one(q);
+    if (b->facet_search_fid) {  // execute_for_candidates: a hybrid search's candidates are its filtered universe (search/mod.rs:254-278)
+        std::vector<const unsigned long long *> dcand;
+        rc = filtered_universes(b, dcand);
+        if (rc == B200_OK) rc = search_facet_search(b, r, dcand);
+        return rc;
+    }
     return B200_OK;
 }
 

@@ -243,5 +243,27 @@ struct FacetSlot {
     uint32_t *out_sum;               // 4 u32: numbers taken, strings taken, FacetHead::min_inv, FacetHead::max_p1
 };
 
+// ---- facet search (facet_search.cu): one request = one (candidate bitmap, field, query)
+constexpr uint32_t FS_MAX_Q = 64;  // B200_FACET_QUERY_MAX: query length in Unicode scalar values
+enum : uint8_t { FS_ALL = 0, FS_PREFIX = 1, FS_EXACT = 2 };
+struct FsTables {  // the staged tables (host_index.h FacetSearchIndex)
+    const uint32_t *chars, *char_off, *csr_off, *csr_key;
+    const uint32_t *pool;
+    const DListRef *lists;
+};
+struct FsReq {
+    const unsigned long long *cand;  // candidates: n_words64 words
+    uint32_t q_off, q_len;           // the query's chars in the batch's query table
+    uint32_t h0, h1;                 // FS_PREFIX / FS_EXACT: the field's hyper-normalised strings
+    uint32_t k0, n_str;              // FS_ALL: the field's level-0 string keys
+    uint32_t max;                    // maxValuesPerFacet (> 0)
+    uint32_t list_base;              // the posting list of level-0 key k is list_base + k (mod 2^32)
+    uint8_t mode, by_count;
+    int8_t k;                        // FS_PREFIX: the OSA budget (0: plain prefix)
+    uint8_t pad;
+    uint32_t *items, *cnt;           // scratch: the walked keys in insertion order and their counts
+    uint32_t *sum;                   // 4 u32: keys walked, hits kept, cut count, offset of the kept hits in the packed outputs
+};
+
 }  // namespace b200
 

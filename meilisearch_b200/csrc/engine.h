@@ -554,6 +554,25 @@ struct Engine {
     int facet_results(const FacetOut &out, const uint16_t *fid, const b200_results &dst, std::vector<std::string> &err);
     int facet_distribution_batch(uint32_t n, const uint64_t *const *candidates, uint64_t n_words, const uint32_t *begin, const uint16_t *fid,
                                  const uint8_t *order, uint32_t max_values, uint32_t cap, const b200_results &dst, int32_t *status);
+    // facet search (facet_search.cu, engine_facet_search.cpp): the staged tables (host_index.h FacetSearchIndex) and per call the
+    // requests, their queries' chars, the candidate bitmaps, the scratch (items and counts) and the packed outputs
+    uint32_t *d_fs_chars = nullptr, *d_fs_char_off = nullptr, *d_fs_csr_off = nullptr, *d_fs_csr_key = nullptr;
+    DevBuf<FsReq> d_fs_reqs;
+    DevBuf<unsigned long long> d_fs_qcand;  // a keyword batch's candidates of its queries with a facet search (slot fs_slot[q])
+    std::vector<int64_t> fs_slot;
+    DevBuf<uint32_t> d_fs_u32;
+    DevBuf<unsigned long long> d_fs_cand;
+    int facet_search_batch(uint32_t n, const uint64_t *const *candidates, uint64_t n_words, const uint16_t *fid, const uint8_t *kind,
+                           const uint32_t *off, const char *query_bytes, const uint8_t *flags, uint32_t max, uint32_t cap, uint32_t *n_out,
+                           uint32_t *key, uint64_t *count, uint32_t *docid, uint8_t *fallback, int32_t *status);
+    // the requests over device bitmaps (nullptr: documents_ids); status is in/out: requests whose status is not 0 are skipped
+    int facet_search_run(uint32_t n, const unsigned long long *const *dcand, const uint16_t *fid, const uint8_t *kind, const uint32_t *off,
+                         const char *query_bytes, const uint8_t *flags, uint32_t max, uint32_t cap, uint32_t *n_out, uint32_t *key,
+                         uint64_t *count, uint32_t *docid, uint8_t *fallback, int32_t *status);
+    // b200_query_batch::facet_search_* of a finished search: query q over dcand[q]; per-query errors land in r->status
+    int search_facet_search(const b200_query_batch *b, b200_results *r, const std::vector<const unsigned long long *> &dcand);
+    // the filtered universe of query q of a semantic or hybrid batch on the device (uploading the caller's bitmaps once each)
+    int filtered_universes(const b200_query_batch *b, std::vector<const unsigned long long *> &dcand);
     ~Engine();
 };
 

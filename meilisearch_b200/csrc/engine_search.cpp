@@ -1778,6 +1778,9 @@ struct KeywordBatch {
     std::vector<RuleBucket> *rule_buckets = nullptr;
     // facets (b200_query_batch::facet_*): computed from each query's candidates where schedule() hands them over
     bool facets = false, facet_outputs = false;  // facet_outputs: facet_fid and every facet_* output are there
+    // facet search (b200_query_batch::facet_search_*): each query's candidates are copied on the device where schedule() hands them
+    // over, into Engine::d_fs_qcand at slot Engine::fs_slot[query]; the facet search runs over them once the batch is done
+    bool fsearch = false;
     Engine::FacetOut fout;
     unsigned n_drivers = 1, lanes_per_driver = 1, n_lanes = 1;
     std::vector<std::vector<std::unique_ptr<Pending>>> lane_acts;  // per lane: the activations of its step in flight
@@ -1881,6 +1884,23 @@ struct KeywordBatch {
                 q.done = true;
             }
         }
+    }
+    int setup_facet_search() {
+        eng.fs_slot.assign(NQ, -1);
+        fsearch = b->mode == 0 && b->facet_search_fid && !has_thr;
+        if (!fsearch) return B200_OK;
+        const size_t W = hix.n_words64;
+        size_t n = 0;
+        for (uint32_t i = 0; i < NQ; i++)
+            if (b->facet_search_fid[i] != 0xFFFF) eng.fs_slot[i] = (int64_t)n++;
+        if (eng.d_fs_qcand.reserve(std::max<size_t>(1, n * W)) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(B200_ERR_CAPACITY, "facet search: the batch's candidate bitmaps (one per query with a facet search) do not fit in device memory");
+        }
+        // a query that never hands over candidates has none
+        CU(cudaMemsetAsync(eng.d_fs_qcand.p, 0, std::max<size_t>(1, n * W) * 8, eng.stream), "zero facet search candidates");
+        CU(cudaStreamSynchronize(eng.stream), "sync");
+        return B200_OK;
     }
     int setup_facets() {
         if (!facets) return B200_OK;
@@ -2601,7 +2621,7 @@ struct KeywordBatch {
             for (auto &pd : q.pendings) cand_q.push_back(Cand{i, pd.get()});
             if (!q.emits.empty()) s.emit_q.push_back(i);
         }
-        if (r->candidates || facets) {
+        if (r->candidates || facets || fsearch) {
             // SearchResult::candidates, copied and counted for the facets before any block freed above can be written again
             std::vector<Engine::FacetJob> fjobs;
             for (auto i : ln.members) {
@@ -2612,6 +2632,11 @@ struct KeywordBatch {
                                        ln.stream),
                        "D2H candidates");
                     ln.lst.d2h_bytes += (size_t)hix.n_words64 * 8;
+                }
+                if (fsearch && eng.fs_slot[i] >= 0) {
+                    CU(cudaMemcpyAsync(eng.d_fs_qcand.p + (size_t)eng.fs_slot[i] * hix.n_words64, q.cand_src, (size_t)hix.n_words64 * 8,
+                                       cudaMemcpyDeviceToDevice, ln.stream),
+                       "D2D facet search candidates");
                 }
                 if (facets && q.status == 0)
                     for (uint32_t k = b->facet_begin[i]; k < b->facet_begin[i + 1]; k++) fjobs.push_back(Engine::FacetJob{q.cand_src, b->facet_fid[k], k});
@@ -3216,7 +3241,7 @@ struct KeywordBatch {
         }
         for (unsigned l = 0; l < n_lanes; l++)
             if (lanes[l].rc < 0) return lanes[l].rc;
-        if (r->candidates || facets)
+        if (r->candidates || facets || fsearch)
             for (unsigned l = 0; l < n_lanes; l++) CU(cudaStreamSynchronize(lanes[l].stream), "sync candidates");
         return B200_OK;
     }
@@ -3793,6 +3818,7 @@ int Engine::keyword_batch(const b200_query_batch *b, b200_results *r, uint32_t o
     int rc = kb.stage_universes();
     if (rc == B200_OK) rc = kb.setup_lanes();
     if (rc == B200_OK) rc = kb.setup_facets();
+    if (rc == B200_OK) rc = kb.setup_facet_search();
     if (rc == B200_OK) rc = kb.drive_waves();
     if (rc == B200_OK) rc = kb.finish_batch();
     return rc;

@@ -91,6 +91,12 @@ Engine::~Engine() {
     for (auto &kv : hix.sort_fields)
         for (auto p : {kv.second.d_key[0], kv.second.d_key[1], kv.second.d_doc_off, kv.second.d_doc_ord, kv.second.d_disp})
             if (p) cudaFree(p);
+    for (auto p : {d_fs_chars, d_fs_char_off, d_fs_csr_off, d_fs_csr_key})
+        if (p) cudaFree(p);
+    d_fs_reqs.release();
+    d_fs_u32.release();
+    d_fs_cand.release();
+    d_fs_qcand.release();
     d_facet_scratch.release();
     d_facet_slots.release();
     d_facet_out.release();
@@ -157,6 +163,8 @@ int Engine::stage_finish() {
         build_host_index(raw_dict_bytes, raw_dict_off, raw_dbs, raw_docids, hix);
         build_sort_fields(raw_dbs[B200_DB_FACET_ID_F64_DOCIDS], raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], hix);
         build_geo_field(raw_dbs[B200_DB_FACET_ID_F64_DOCIDS], raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], hix);
+        build_facet_search(raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], raw_dbs[B200_DB_FACET_ID_NORMALIZED_STRING_STRINGS],
+                           raw_dbs[B200_DB_FIELD_ID_DOCID_FACET_STRINGS], hix);
     } catch (const std::exception &e) {
         return fail(B200_ERR_INVALID, e.what());
     }
@@ -196,6 +204,21 @@ int Engine::stage_finish() {
         std::vector<uint32_t>().swap(f.doc_off);
         std::vector<uint32_t>().swap(f.doc_ord);
         std::vector<uint32_t>().swap(f.disp);
+    }
+    // facet search: the hyper-normalised strings as chars and the keys each one walks (the keys' posting lists are in the pool,
+    // counted above)
+    {
+        FacetSearchIndex &fs = hix.fsearch;
+        auto src = [](const std::vector<uint32_t> &v) { return v.empty() ? nullptr : v.data(); };  // upload() allocates one element for none
+        CU(upload(&d_fs_chars, src(fs.chars), fs.chars.size()), "upload facet search strings");
+        CU(upload(&d_fs_char_off, src(fs.char_off), fs.char_off.size()), "upload facet search strings");
+        CU(upload(&d_fs_csr_off, src(fs.csr_off), fs.csr_off.size()), "upload facet search keys");
+        CU(upload(&d_fs_csr_key, src(fs.csr_key), fs.csr_key.size()), "upload facet search keys");
+        stats.hbm_bytes_staged += (fs.chars.size() + fs.char_off.size() + fs.csr_off.size() + fs.csr_key.size()) * 4;
+        std::vector<uint32_t>().swap(fs.chars);
+        std::vector<uint32_t>().swap(fs.char_off);
+        std::vector<uint32_t>().swap(fs.csr_off);
+        std::vector<uint32_t>().swap(fs.csr_key);
     }
     // GeoSort points: lat_lng_to_xyz (lib.rs:397-404) and cos(lat) with the host's libm, as the reference computes them
     {

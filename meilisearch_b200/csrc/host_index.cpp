@@ -8,6 +8,7 @@
 #include <charconv>
 #include <cstdlib>
 #include <stdexcept>
+#include <set>
 #include <thread>
 
 namespace b200 {
@@ -62,6 +63,32 @@ uint32_t cbo_decode_append(const uint8_t *p, size_t n, std::vector<uint32_t> &ou
     return (uint32_t)(out.size() - start);
 }
 
+// Append one posting list (ascending docids) to the pool.  A list is stored as a dense bitmap over the docid space when card >
+// n_docs / 128 (B200_DENSE_DIV): a bitmap costs n_docs / 8 bytes, i.e. at most 4x the sorted-docid form at that density, and turns
+// the scatter of the list into a coalesced gather by universe row instead of one random row lookup per docid (DESIGN.md §2).
+uint32_t dense_min_card(const HostIndex &ix) {
+    uint32_t dense_div = 128;
+    if (const char *env = getenv("B200_DENSE_DIV")) dense_div = (uint32_t)std::max(8, atoi(env));
+    return ix.n_docs / dense_div;
+}
+void append_list(HostIndex &ix, const uint32_t *src, uint32_t c, uint32_t dense_min) {
+    if (ix.pool.size() & 1) ix.pool.push_back(0);  // keep every list 8-byte aligned
+    ListRef r{ix.pool.size(), c, 0};
+    if (c > dense_min && c > 64) {
+        r.dense = 1;
+        size_t base = ix.pool.size();
+        ix.pool.resize(base + 2 * (size_t)ix.n_words64, 0);
+        uint64_t *words = reinterpret_cast<uint64_t *>(ix.pool.data() + base);
+        for (uint32_t k = 0; k < c; k++) {
+            uint32_t d = src[k];
+            if (d < ix.n_docs) words[d >> 6] |= 1ull << (d & 63);
+        }
+    } else {
+        ix.pool.insert(ix.pool.end(), src, src + c);
+    }
+    ix.lists.push_back(r);
+}
+
 struct Builder {
     HostIndex &ix;
     const RawDb *dbs_base = nullptr;
@@ -99,12 +126,7 @@ struct Builder {
         for (auto &e : errs)
             if (!e.empty()) throw std::runtime_error(e);
         uint32_t first = (uint32_t)ix.lists.size();
-        // A list is stored as a dense bitmap over the docid space when card > n_docs / 128 (B200_DENSE_DIV): a bitmap costs
-        // n_docs / 8 bytes, i.e. at most 4x the sorted-docid form at that density, and turns the scatter of the list into a coalesced
-        // gather by universe row instead of one random row lookup per docid (DESIGN.md §2).
-        uint32_t dense_div = 128;
-        if (const char *env = getenv("B200_DENSE_DIV")) dense_div = (uint32_t)std::max(8, atoi(env));
-        uint32_t dense_min = ix.n_docs / dense_div;
+        const uint32_t dense_min = dense_min_card(ix);
         for (unsigned t = 0; t < nt; t++) {
             size_t at = 0;
             for (uint32_t c : cards[t]) {
@@ -112,23 +134,8 @@ struct Builder {
                     ix.lists.push_back(ListRef{0, 0, 0});
                     continue;
                 }
-                const uint32_t *src = parts[t].data() + at;
+                append_list(ix, parts[t].data() + at, c, dense_min);
                 at += c;
-                if (ix.pool.size() & 1) ix.pool.push_back(0);  // keep every list 8-byte aligned
-                ListRef r{ix.pool.size(), c, 0};
-                if (c > dense_min && c > 64) {
-                    r.dense = 1;
-                    size_t base = ix.pool.size();
-                    ix.pool.resize(base + 2 * (size_t)ix.n_words64, 0);
-                    uint64_t *words = reinterpret_cast<uint64_t *>(ix.pool.data() + base);
-                    for (uint32_t k = 0; k < c; k++) {
-                        uint32_t d = src[k];
-                        if (d < ix.n_docs) words[d >> 6] |= 1ull << (d & 63);
-                    }
-                } else {
-                    ix.pool.insert(ix.pool.end(), src, src + c);
-                }
-                ix.lists.push_back(r);
             }
             std::vector<uint32_t>().swap(parts[t]);
         }
@@ -497,6 +504,226 @@ void build_geo_field(const RawDb &f64_db, const RawDb &string_db, HostIndex &ix)
         if (!(ix.base_ub[d >> 6] >> (d & 63) & 1)) continue;  // not in documents_ids
         g.ub[d >> 6] |= 1ull << (d & 63);
         g.n_geo++;
+    }
+}
+
+bool parse_json_string_array(const uint8_t *s, size_t n, std::vector<std::string> &out) {
+    out.clear();
+    size_t i = 0;
+    auto ws = [&]() {
+        while (i < n && (s[i] == ' ' || s[i] == '\t' || s[i] == '\n' || s[i] == '\r')) i++;
+    };
+    auto hex4 = [&](uint32_t &v) {
+        if (i + 4 > n) return false;
+        v = 0;
+        for (int k = 0; k < 4; k++) {
+            const uint8_t c = s[i++];
+            const int d = c >= '0' && c <= '9' ? c - '0' : c >= 'a' && c <= 'f' ? c - 'a' + 10 : c >= 'A' && c <= 'F' ? c - 'A' + 10 : -1;
+            if (d < 0) return false;
+            v = v << 4 | (uint32_t)d;
+        }
+        return true;
+    };
+    auto put_utf8 = [](std::string &o, uint32_t c) {
+        if (c < 0x80) {
+            o += (char)c;
+        } else if (c < 0x800) {
+            o += (char)(0xC0 | c >> 6);
+            o += (char)(0x80 | (c & 63));
+        } else if (c < 0x10000) {
+            o += (char)(0xE0 | c >> 12);
+            o += (char)(0x80 | (c >> 6 & 63));
+            o += (char)(0x80 | (c & 63));
+        } else {
+            o += (char)(0xF0 | c >> 18);
+            o += (char)(0x80 | (c >> 12 & 63));
+            o += (char)(0x80 | (c >> 6 & 63));
+            o += (char)(0x80 | (c & 63));
+        }
+    };
+    ws();
+    if (i >= n || s[i++] != '[') return false;
+    ws();
+    if (i < n && s[i] == ']') {
+        i++;
+        ws();
+        return i == n;
+    }
+    for (;;) {
+        ws();
+        if (i >= n || s[i++] != '"') return false;
+        std::string v;
+        for (;;) {
+            if (i >= n) return false;
+            const uint8_t c = s[i++];
+            if (c == '"') break;
+            if (c < 0x20) return false;
+            if (c != '\\') {
+                v += (char)c;
+                continue;
+            }
+            if (i >= n) return false;
+            const uint8_t e = s[i++];
+            uint32_t cp = 0;
+            switch (e) {
+                case '"': v += '"'; break;
+                case '\\': v += '\\'; break;
+                case '/': v += '/'; break;
+                case 'b': v += '\b'; break;
+                case 'f': v += '\f'; break;
+                case 'n': v += '\n'; break;
+                case 'r': v += '\r'; break;
+                case 't': v += '\t'; break;
+                case 'u':
+                    if (!hex4(cp)) return false;
+                    if (cp >= 0xD800 && cp < 0xDC00) {  // a surrogate pair
+                        uint32_t lo = 0;
+                        if (i + 2 > n || s[i] != '\\' || s[i + 1] != 'u') return false;
+                        i += 2;
+                        if (!hex4(lo) || lo < 0xDC00 || lo >= 0xE000) return false;
+                        cp = 0x10000 + ((cp - 0xD800) << 10) + (lo - 0xDC00);
+                    } else if (cp >= 0xDC00 && cp < 0xE000) {
+                        return false;
+                    }
+                    put_utf8(v, cp);
+                    break;
+                default: return false;
+            }
+        }
+        out.push_back(std::move(v));
+        ws();
+        if (i >= n) return false;
+        if (s[i] == ',') {
+            i++;
+            continue;
+        }
+        if (s[i++] != ']') return false;
+        ws();
+        return i == n;
+    }
+}
+
+bool utf8_decode(const uint8_t *s, size_t n, std::vector<uint32_t> &out) {
+    out.clear();
+    for (size_t i = 0; i < n;) {
+        const uint8_t c = s[i];
+        const int len = c < 0x80 ? 1 : (c >> 5) == 6 ? 2 : (c >> 4) == 14 ? 3 : (c >> 3) == 30 ? 4 : 0;
+        if (!len || i + len > n) return false;
+        uint32_t cp = len == 1 ? c : (c & (0x7F >> len));
+        for (int k = 1; k < len; k++) {
+            if ((s[i + k] & 0xC0) != 0x80) return false;
+            cp = cp << 6 | (s[i + k] & 63);
+        }
+        static const uint32_t least[5] = {0, 0, 0x80, 0x800, 0x10000};  // overlong forms are not UTF-8
+        if (cp < least[len] || cp > 0x10FFFF || (cp >= 0xD800 && cp < 0xE000)) return false;
+        out.push_back(cp);
+        i += len;
+    }
+    return true;
+}
+
+void build_facet_search(const RawDb &string_db, const RawDb &norm_db, const RawDb &orig_db, HostIndex &ix) {
+    FacetSearchIndex &fs = ix.fsearch;
+    fs = FacetSearchIndex();
+    // the level-0 string keys, their posting lists (appended to the pool in key order) and smallest docids
+    std::map<std::pair<uint16_t, std::string>, uint32_t> key_of;
+    std::map<uint16_t, std::pair<uint32_t, uint32_t>> range;  // fid -> (first key, number of keys)
+    std::map<uint16_t, uint32_t> list0;  // fid -> the list id of its first level-0 string key
+    const uint32_t dense_min = dense_min_card(ix);
+    std::vector<uint32_t> docs, kept, chars;
+    // the fields facet search can reach: those with normalised strings (a field without them has no FST)
+    std::set<uint16_t> searchable;
+    for (uint64_t i = 0; i < norm_db.n; i++)
+        if (norm_db.koff[i + 1] - norm_db.koff[i] >= 2) {
+            const uint8_t *k = norm_db.keys.data() + norm_db.koff[i];
+            searchable.insert((uint16_t)(k[0] << 8 | k[1]));
+        }
+    for (uint64_t i = 0; i < string_db.n; i++) {
+        const uint8_t *k = string_db.keys.data() + string_db.koff[i];
+        const size_t kn = string_db.koff[i + 1] - string_db.koff[i];
+        if (kn < 3 || k[2] != 0) continue;
+        const uint16_t fid = (uint16_t)(k[0] << 8 | k[1]);
+        const uint32_t at = (uint32_t)fs.key.size();
+        auto r = range.emplace(fid, std::make_pair(at, 0u)).first;
+        r->second.second++;
+        if (!searchable.count(fid)) {  // no list, key or original for it: a placeholder keeps the key positions
+            fs.key.emplace_back();
+            fs.min_doc.push_back(0);
+            continue;
+        }
+        if (r->second.second == 1) list0[fid] = (uint32_t)ix.lists.size();
+        docs.clear();
+        cbo_decode_append(string_db.vals.data() + string_db.voff[i] + 1, string_db.voff[i + 1] - string_db.voff[i] - 1, docs);
+        kept.clear();
+        for (uint32_t d : docs)
+            if (d < ix.n_docs) kept.push_back(d);
+        append_list(ix, kept.data(), (uint32_t)kept.size(), dense_min);
+        fs.key.emplace_back((const char *)k + 3, kn - 3);
+        fs.min_doc.push_back(docs.empty() ? 0 : docs[0]);
+        key_of.emplace(std::make_pair(fid, fs.key.back()), at);
+    }
+    // the original naming each key: field_id_docid_facet_strings at (fid, smallest docid, key)
+    fs.has_orig.assign(fs.key.size(), 0);
+    fs.orig.assign(fs.key.size(), std::string());
+    for (auto &kv : key_of) {
+        std::string probe(6, '\0');
+        const uint32_t d = fs.min_doc[kv.second];
+        probe[0] = (char)(kv.first.first >> 8);
+        probe[1] = (char)(kv.first.first & 255);
+        for (int b = 0; b < 4; b++) probe[2 + b] = (char)(d >> (24 - 8 * b) & 255);
+        probe += kv.first.second;
+        uint64_t lo = 0, hi = orig_db.n;
+        while (lo < hi) {
+            const uint64_t mid = (lo + hi) / 2;
+            const size_t mn = orig_db.koff[mid + 1] - orig_db.koff[mid];
+            const int c = memcmp(orig_db.keys.data() + orig_db.koff[mid], probe.data(), std::min(mn, probe.size()));
+            if (c < 0 || (c == 0 && mn < probe.size()))
+                lo = mid + 1;
+            else
+                hi = mid;
+        }
+        if (lo < orig_db.n && orig_db.koff[lo + 1] - orig_db.koff[lo] == probe.size() &&
+            memcmp(orig_db.keys.data() + orig_db.koff[lo], probe.data(), probe.size()) == 0) {
+            fs.has_orig[kv.second] = 1;
+            fs.orig[kv.second].assign((const char *)orig_db.vals.data() + orig_db.voff[lo], orig_db.voff[lo + 1] - orig_db.voff[lo]);
+        }
+    }
+    // the hyper-normalised strings, field by field in key order, and the keys each one walks
+    std::vector<std::string> set;
+    for (uint64_t i = 0; i < norm_db.n; i++) {
+        const uint8_t *k = norm_db.keys.data() + norm_db.koff[i];
+        const size_t kn = norm_db.koff[i + 1] - norm_db.koff[i];
+        if (kn < 2) throw std::runtime_error("stage: facet_id_normalized_string_strings key shorter than its field id");
+        const uint16_t fid = (uint16_t)(k[0] << 8 | k[1]);
+        if (!parse_json_string_array(norm_db.vals.data() + norm_db.voff[i], norm_db.voff[i + 1] - norm_db.voff[i], set))
+            throw std::runtime_error("stage: a facet_id_normalized_string_strings value is not a JSON array of strings");
+        std::sort(set.begin(), set.end());  // a BTreeSet<String>: byte order, no duplicates, whatever order the bytes list them in
+        set.erase(std::unique(set.begin(), set.end()), set.end());
+        const uint32_t h = (uint32_t)fs.char_off.size() - 1;
+        auto ins = fs.fields.emplace(fid, FacetSearchField());
+        FacetSearchField &f = ins.first->second;
+        if (ins.second) {
+            f.h0 = h;
+            auto r = range.find(fid);
+            if (r != range.end()) {
+                f.k0 = r->second.first;
+                f.n_str = r->second.second;
+                f.list0 = list0[fid];
+            }
+        } else if (f.h1 != h) {
+            throw std::runtime_error("stage: facet_id_normalized_string_strings keys not in LMDB order");
+        }
+        f.h1 = h + 1;
+        if (!utf8_decode(k + 2, kn - 2, chars)) throw std::runtime_error("stage: a facet_id_normalized_string_strings key is not valid UTF-8");
+        fs.chars.insert(fs.chars.end(), chars.begin(), chars.end());
+        fs.char_off.push_back((uint32_t)fs.chars.size());
+        for (const std::string &s : set) {
+            auto it = key_of.find(std::make_pair(fid, s));
+            if (it == key_of.end()) break;  // the reference logs the missing key and skips the rest of this entry
+            fs.csr_key.push_back(it->second);
+        }
+        fs.csr_off.push_back((uint32_t)fs.csr_key.size());
+        f.n_entries += fs.csr_off[h + 1] - fs.csr_off[h];
     }
 }
 

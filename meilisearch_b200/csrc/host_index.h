@@ -85,6 +85,26 @@ struct GeoField {
     uint64_t n_geo = 0;
 };
 
+// Facet search (facet_search.cu) over every field with facet_id_normalized_string_strings entries.  The hyper-normalised strings of
+// all fields are one table in byte order per field, decoded to Unicode scalar values (chars / char_off, one u32 per char); string h
+// walks the level-0 string keys csr_key[csr_off[h] .. csr_off[h + 1]) (positions among the staged level-0 keys of
+// facet_id_string_docids, cut at the first key that database lacks; a set is read as the BTreeSet it is: sorted, deduplicated).
+// Only the fields with such strings get their keys' posting lists (FacetSearchField::list0), smallest docids and originals in
+// field_id_docid_facet_strings (has_orig 0: none).
+struct FacetSearchField {
+    uint32_t h0 = 0, h1 = 0;  // its hyper-normalised strings
+    uint32_t k0 = 0, n_str = 0;  // its level-0 string keys [k0, k0 + n_str)
+    uint32_t n_entries = 0;  // csr_off[h1] - csr_off[h0]
+    uint32_t list0 = 0;      // the posting list of key k0 + i is list0 + i
+};
+struct FacetSearchIndex {
+    std::map<uint16_t, FacetSearchField> fields;
+    std::vector<uint32_t> chars, char_off{0}, csr_off{0}, csr_key;  // released after upload
+    std::vector<uint32_t> min_doc;      // per level-0 string key
+    std::vector<uint8_t> has_orig;
+    std::vector<std::string> orig, key; // per level-0 string key: its original (when has_orig) and the key itself
+};
+
 struct HostIndex {
     // dictionary
     std::vector<uint8_t> dict_bytes;
@@ -111,6 +131,7 @@ struct HostIndex {
     std::map<uint32_t, uint32_t> fwc_list;  // fid<<8|count -> list
     std::map<uint16_t, SortField> sort_fields;  // faceted fields (fid -> SortField)
     GeoField geo;
+    FacetSearchIndex fsearch;
     // list id of key i of database db = db_first[db] + i (keys in LMDB order); db_keys[db] = number of staged keys.
     // (word_pair_proximity keys naming unknown words are dropped at staging: for that db the mapping only holds when none was.)
     uint32_t db_first[10] = {0}, db_keys[10] = {0};
@@ -215,5 +236,13 @@ std::string rust_f64_display(double v);
 // Read every document's point into out.geo (after build_host_index; out.geo.lat_fid / lng_fid set, or nothing to do).  Throws
 // std::runtime_error for a document with one coordinate only or a string coordinate that does not parse as f64.
 void build_geo_field(const RawDb &f64_db, const RawDb &string_db, HostIndex &out);
+// Build out.fsearch from facet_id_string_docids, facet_id_normalized_string_strings and field_id_docid_facet_strings, appending the
+// level-0 string keys' posting lists to the pool (after build_host_index, before the pool is uploaded).  Throws std::runtime_error
+// on a malformed key or a value that is not a JSON array of strings.
+void build_facet_search(const RawDb &string_db, const RawDb &norm_db, const RawDb &orig_db, HostIndex &out);
+// The JSON array of strings `s` (serde_json's output for a BTreeSet<String>, escapes included), false when it is not one
+bool parse_json_string_array(const uint8_t *s, size_t n, std::vector<std::string> &out);
+// The Unicode scalar values of UTF-8 bytes; false when they are not UTF-8 (overlong forms and surrogates included)
+bool utf8_decode(const uint8_t *s, size_t n, std::vector<uint32_t> &out);
 
 }  // namespace b200

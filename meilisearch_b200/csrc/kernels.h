@@ -41,6 +41,11 @@ cudaError_t launch_geo_filter(cudaStream_t s, const unsigned long long *geo, con
 // facet.cu: counts of every slot's values over its candidates (FacetSlot scratch zero at launch), then one CTA per slot selects the
 // entries the reference's facet_values returns
 cudaError_t launch_facet(cudaStream_t s, const FacetSlot *slots, uint32_t n_slots, uint32_t n_words, uint32_t n_docs);
+// facet_search.cu: match, count and select of `n` requests; the kept hits of request r are (out_key, out_cnt)[sum[3] .. + sum[1]),
+// packed through *cursor (zero at launch).  max_items: the largest request's scratch.
+cudaError_t launch_facet_search_match(cudaStream_t s, const FsTables &t, const FsReq *reqs, uint32_t n, const uint32_t *q_chars);
+cudaError_t launch_facet_search_count(cudaStream_t s, const FsTables &t, const FsReq *reqs, uint32_t n, uint32_t max_items, uint32_t n_words);
+cudaError_t launch_facet_search_select(cudaStream_t s, const FsReq *reqs, uint32_t n, uint32_t *out_key, uint32_t *out_cnt, uint32_t *cursor);
 cudaError_t launch_vec_dist(cudaStream_t s, int n_ctas, int qt, const void *mat_fp16, const float *inv_norm, const uint32_t *docids,
                             uint64_t n_rows, uint32_t d, const float *queries, const float *q_inv_norm, const unsigned long long *cand,
                             uint64_t n_cand_words, float *dist);
