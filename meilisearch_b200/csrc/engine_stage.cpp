@@ -429,6 +429,10 @@ int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t l
     }
     if (n_q == 0) return B200_OK;
     const uint64_t N = dix.emb_n;
+    if (N == 0 && !sharded) {  // an empty store: no hits (the batched path could not even describe a matrix of 0 rows to TMA)
+        memset(n_out, 0, (size_t)n_q * 4);
+        return B200_OK;
+    }
     const uint32_t tie_cap = 1024;
     const uint32_t QT = 8;  // queries per scan pass
     uint32_t chunk = std::min<uint32_t>(n_q, 64);  // queries whose distance rows are resident at once

@@ -1130,7 +1130,7 @@ __global__ void __launch_bounds__(256) vec_dist_kernel(const __half *__restrict_
             for (int q = 0; q < QT; q++) {
                 float dd = 0.f;
                 float pn = vn * q_inv_norm[q];
-                if (pn > 0.f && isfinite(pn)) {
+                if (norm_rule_ok(pn)) {
                     float cs = acc[q] * pn;
                     cs = fminf(1.f, fmaxf(-1.f, cs));
                     dd = (1.f - cs) * 0.5f;
@@ -1234,7 +1234,57 @@ __global__ void __launch_bounds__(1024) topk_select_kernel(const float *__restri
         }
     }
     __syncthreads();
-    const uint32_t n_lt = min(s_count_lt, k), n_eq = min(s_count_eq, tie_cap);
+    uint32_t n_lt = min(s_count_lt, k), n_eq = min(s_count_eq, tie_cap);
+    if (s_count_eq > tie_cap && remaining > 0) {
+        // More rows share the k-th distance than the tie buffer holds (a zero query, duplicated embeddings): the buffer kept them
+        // in arrival order.  Select the `remaining` smallest docids among them instead, by a second radix select on the docids of
+        // the tied rows, and write those into the free slots [n_lt, k) of the main output; the tie buffer is then unused.
+        uint32_t dprefix = 0, dmask = 0, dremaining = remaining;
+        for (int pass = 0; pass < 4; pass++) {
+            for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0;
+            __syncthreads();
+            for (uint64_t r = threadIdx.x; r < n_rows; r += blockDim.x) {
+                if (__float_as_uint(dq[r]) != prefix) continue;
+                const uint32_t doc = docids[r];
+                if ((doc & dmask) == dprefix) atomicAdd(&hist[(doc >> shifts[pass]) & 255u], 1u);
+            }
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                uint32_t acc = 0, sel = 255;
+                for (uint32_t i = 0; i < 256; i++) {  // the tied rows number at least `remaining`: some bin is reached
+                    if (acc + hist[i] >= dremaining) {
+                        sel = i;
+                        break;
+                    }
+                    acc += hist[i];
+                }
+                s_prefix = dprefix | (sel << shifts[pass]);
+                s_remaining = dremaining - acc;
+            }
+            __syncthreads();
+            dprefix = s_prefix;
+            dremaining = s_remaining;
+            dmask |= 255u << shifts[pass];
+            __syncthreads();
+        }
+        // dprefix = the remaining-th smallest tied docid; `dremaining` rows with that docid are still wanted (duplicate docids
+        // carry the same key, so any of them will do)
+        if (threadIdx.x == 0) {
+            s_count_lt = 0;
+            s_count_eq = 0;
+        }
+        __syncthreads();
+        for (uint64_t r = threadIdx.x; r < n_rows; r += blockDim.x) {
+            if (__float_as_uint(dq[r]) != prefix) continue;
+            const uint32_t doc = docids[r];
+            if (doc > dprefix || (doc == dprefix && atomicAdd(&s_count_eq, 1u) >= dremaining)) continue;
+            const uint32_t at = n_lt + atomicAdd(&s_count_lt, 1u);
+            od[at] = dq[r];
+            oi[at] = doc;
+        }
+        n_lt = k;
+        n_eq = 0;
+    }
     for (uint32_t i = n_lt + threadIdx.x; i < k; i += blockDim.x) od[i] = 3.0f;           // unused slots: "no candidate"
     for (uint32_t i = n_eq + threadIdx.x; i < tie_cap; i += blockDim.x) od[k + i] = 3.0f;
     if (threadIdx.x == 0) {

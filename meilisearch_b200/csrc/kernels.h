@@ -55,6 +55,11 @@ cudaError_t launch_topk(cudaStream_t s, uint32_t n_q, const float *dist, const u
                         uint32_t n_slices, float *part_dist, uint32_t *part_ids, uint32_t *part_n, float *out_dist, uint32_t *out_ids,
                         uint32_t *out_n);
 
+// The norm rule of arroy/hannoy `Cosine`: the distance is 0 unless |q||v| > f32::EPSILON = 2^-23.  The kernels hold inverse norms
+// (0 for a zero vector), so the test is on their product pn: a cosine only for 0 < pn < 2^23.  A NaN pn (0 x inf) fails it too.
+constexpr float VEC_PN_MAX = 8388608.f;
+__host__ __device__ inline bool norm_rule_ok(float pn) { return pn > 0.f && pn < VEC_PN_MAX; }
+
 // staging of the vector store: f32 rows -> fp16 rows + inverse norms; inverse norms of fp16 rows
 cudaError_t launch_emb_from_f32(cudaStream_t s, const float *in, void *out_fp16, float *inv_norm, uint64_t n, uint32_t d);
 cudaError_t launch_emb_norm_f16(cudaStream_t s, const void *rows_fp16, float *inv_norm, uint64_t n, uint32_t d);

@@ -8,7 +8,8 @@
 // Per CTA (one per SM, 256 threads):
 //   warp 0     TMA producer: the query tile [64 x d] once (A operand, resident: d/64 blocks of 8 KB, 128B-swizzled, K-major),
 //              then matrix blocks [128 rows x 64 halfs] = two row tiles through a 4-stage ring (B operand)
-//   warp 1     stages each row tile's docids (filtered rows marked) and inverse norms in shared memory, one tile ahead
+//   warp 1     stages each row tile's docids (filtered rows marked) and inverse norms (NaN for rows the norm rule may send to
+//              distance 0) in shared memory, one tile ahead
 //   warps 2-3  epilogue: lane = query; reads the tile's 64 fp32 dots from the accumulator staging buffer, distance, compare with
 //              the query's running threshold, append survivors to the query's candidate run in L2-resident scratch; a
 //              warp-cooperative bitonic sort compacts a run to its k best whenever it fills up, which tightens the threshold.
@@ -230,6 +231,7 @@ __global__ void __launch_bounds__(256, 1)
     // row metadata ring: static shared memory, so that the epilogue reads it with (vectorisable) LDS instead of generic loads
     __shared__ __align__(16) uint32_t s_doc[META_BUFS * GN];
     __shared__ __align__(16) float s_scale[META_BUFS * GN];
+    __shared__ __align__(16) float s_norm[META_BUFS * GN];  // the rows' own inverse norms, for the NaN-scaled ones
 
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t qtile = blockIdx.x % n_qtiles, group = blockIdx.x / n_qtiles;
@@ -276,6 +278,15 @@ __global__ void __launch_bounds__(256, 1)
                 }
             }
     } else if (warp == 1) {
+        // The fast reject of the epilogue compares dot x inverse row norm with a bound derived from a real cosine; it knows nothing
+        // of the norm rule (distance 0 unless 0 < pn < 2^23).  Rows that rule can send to 0 for some query of the tile bypass the
+        // reject: for a query with a non-zero inverse norm qn that is a zero row, or one with scale * qn >= 2^23, and the product is
+        // monotonic in qn, so the tile's largest qn decides.  (Zero queries have no reject bound at all.)  Such a row is staged
+        // with a NaN scale: v * NaN < bound is false for every query, and the exact test reads the row's own scale.
+        float qmax = 0.f;
+        for (uint32_t i = lane; i < GM; i += 32) qmax = fmaxf(qmax, q_inv_norm[qtile * GM + i]);
+#pragma unroll
+        for (int o = 16; o; o >>= 1) qmax = fmaxf(qmax, __shfl_xor_sync(0xffffffffu, qmax, o));
         uint32_t n = 0;
         for (uint64_t t = tile_lo; t < tile_hi; t++, n++) {
             const uint32_t mb = n % META_BUFS, mph = (n / META_BUFS) & 1;
@@ -284,15 +295,16 @@ __global__ void __launch_bounds__(256, 1)
             for (int h = 0; h < GN / 32; h++) {
                 const uint64_t r = t * GN + (uint32_t)h * 32u + lane;
                 uint32_t doc = 0xffffffffu;
-                float sc = 0.f;
+                float sc = 0.f, nrm = 0.f;
                 if (r < n_rows) {
                     doc = __ldg(docids + r);
-                    sc = __ldg(inv_norm + r);
-                    if (!(sc > 0.f)) sc = __int_as_float(0x7f800000);  // zero norm: v*inf is NaN/inf, never fast-rejected; pn not finite -> distance 0
+                    sc = nrm = __ldg(inv_norm + r);
+                    if (!(sc > 0.f && sc * qmax < VEC_PN_MAX)) sc = __int_as_float(0x7fffffff);
                     if (cand && !((doc >> 6) < n_cand_words && ((__ldg(cand + (doc >> 6)) >> (doc & 63)) & 1))) doc = 0xffffffffu;
                 }
                 s_doc[mb * GN + h * 32 + lane] = doc;
                 s_scale[mb * GN + h * 32 + lane] = sc;
+                s_norm[mb * GN + h * 32 + lane] = nrm;
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(meta_full + mb);
@@ -384,8 +396,9 @@ __global__ void __launch_bounds__(256, 1)
             const uint32_t mb = n % META_BUFS, mph = (n / META_BUFS) & 1;
             mbar_wait(meta_full + mb, mph);
             const uint32_t *tdoc = s_doc + mb * GN;
-            const float *tscale = s_scale + mb * GN;
-            // pass 1, branch-free: which of the 64 rows can possibly beat this query's threshold ("dot x inverse row norm" space)
+            const float *tscale = s_scale + mb * GN, *tnorm = s_norm + mb * GN;
+            // pass 1, branch-free: which of the 64 rows can possibly beat this query's threshold ("dot x inverse row norm" space;
+            // a NaN scale, a row the norm rule may send to 0, always passes)
             uint32_t m_lo = 0, m_hi = 0;
 #pragma unroll
             for (int j = 0; j < 32; j++) {
@@ -405,7 +418,13 @@ __global__ void __launch_bounds__(256, 1)
                 if ((mm >> (j & 31)) & 1u) {
                     const float dot = col[j * ACC_LD];
                     const uint32_t doc = tdoc[j];
-                    const float pn = tscale[j] * qn;
+                    float pn = tscale[j] * qn;
+                    // A row staged with a finite scale has 0 <= pn <= scale x (the tile's largest qn) < 2^23, so for it the norm
+                    // rule is pn > 0.  A NaN scale (warp 1) takes the rule with the row's own scale.
+                    if (pn != pn) {
+                        pn = tnorm[j] * qn;
+                        pn = pn < VEC_PN_MAX ? pn : 0.f;
+                    }
                     float dd = 0.f;
                     if (pn > 0.f && isfinite(pn)) {
                         float cs = dot * pn;

@@ -528,27 +528,29 @@ def test_prefix_search_disabled_matches_oracle(mb, synth):
 
 
 def test_nns_many_ties_and_duplicate_docids(mb, synth):
-    """more equal-distance rows than the selection's tie buffer, and several embeddings per document"""
+    """more equal-distance rows than the selection's tie buffer, and several embeddings per document; with docids in row order
+    and permuted (then row order says nothing about which tied rows have the smallest docids)"""
     from oracle.pyoracle import OracleIndex
 
     rng = np.random.default_rng(4)
     n, d = 6000, 64
     emb = rng.standard_normal((n, d)).astype(np.float16).astype(np.float32)
     emb[1000:3500] = emb[999]                      # 2501 identical rows: a tie far longer than any top-k
-    docids = np.arange(n, dtype=np.uint32)
-    docids[4000:4200] = docids[100:300]            # 200 documents own two embeddings each
     ix, o = mb.Index(synth), OracleIndex(synth)
-    ix.set_embeddings(emb, docids)
-    o.set_embeddings(emb, docids)
     q = np.stack([emb[999], emb[150], rng.standard_normal(d).astype(np.float32)])
-    for k in (10, 100):
-        ids, dist, cnt = ix.nns_by_vector(q, k)
-        for i in range(len(q)):
-            oid, od = o.nns(q[i], k)
-            assert cnt[i] == len(oid)
-            assert np.allclose(dist[i, : cnt[i]], od, rtol=1e-4, atol=2e-6)
-            # inside a run of equal distances the order is ascending docid on both sides
-            assert list(ids[i, : cnt[i]]) == list(oid), (i, k)
+    for layout in ("row order", "permuted"):
+        docids = np.arange(n, dtype=np.uint32) if layout == "row order" else rng.permutation(n).astype(np.uint32)
+        docids[4000:4200] = docids[100:300]        # 200 documents own two embeddings each
+        ix.set_embeddings(emb, docids)
+        o.set_embeddings(emb, docids)
+        for k in (10, 100):
+            ids, dist, cnt = ix.nns_by_vector(q, k)
+            for i in range(len(q)):
+                oid, od = o.nns(q[i], k)
+                assert cnt[i] == len(oid)
+                assert np.allclose(dist[i, : cnt[i]], od, rtol=1e-4, atol=2e-6)
+                # inside a run of equal distances the order is ascending docid on both sides
+                assert list(ids[i, : cnt[i]]) == list(oid), (layout, i, k)
 
 
 def test_path_table_growth(mb):
