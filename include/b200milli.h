@@ -434,6 +434,9 @@ typedef struct {
     uint64_t arena_peak_bytes;    /* high-water mark of the per-batch level storage (universes + bucket columns) */
     uint64_t eval_class_launches[9]; /* eval_dp launches per DP-table class: <= 16 / 24 / 40 / 56 / 80 / 112 / 160 / 216 slots in shared memory, [8] = global matrices */
     uint64_t eval_class_tiles[9];    /* 128-row tiles evaluated per class */
+    uint64_t lev_terms;           /* term derivation: distinct terms derived */
+    uint64_t lev_items;           /* term derivation: lev_match work items (one CTA each) */
+    uint64_t lev_pairs;           /* term derivation: (term, dictionary word) pairs the work items cover */
 } b200_stats;
 int b200_get_stats(b200_index *, b200_stats *out);
 int b200_reset_stats(b200_index *);

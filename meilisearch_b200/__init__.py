@@ -71,7 +71,8 @@ class _Stats(C.Structure):
                 ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 15),
                 ("kernel_count", C.c_uint64 * 15), ("kernel_bytes", C.c_uint64 * 15), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
                 ("hbm_bytes_staged", C.c_uint64), ("deferred", C.c_uint64), ("arena_peak_bytes", C.c_uint64),
-                ("eval_class_launches", C.c_uint64 * 9), ("eval_class_tiles", C.c_uint64 * 9)]
+                ("eval_class_launches", C.c_uint64 * 9), ("eval_class_tiles", C.c_uint64 * 9),
+                ("lev_terms", C.c_uint64), ("lev_items", C.c_uint64), ("lev_pairs", C.c_uint64)]
 
 
 KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort", "geo", "geo_filter", "facet", "facet_search"]

@@ -14,6 +14,11 @@ struct DListRef {  // mirrors host ListRef
 constexpr int LEV_MAX_Q = 64;        // longest query word handled on device (bytes)
 constexpr int LEV_TERMS_PER_CTA = 32;
 constexpr int LEV_REC_CAP = 2048;    // match records (32 words each) per term
+// Record slots per term.  A term's work items scan at most LEV_MAX_RANGES disjoint word ranges (first bytes q[0] and q[1], the
+// 2-byte prefixes (c, q[1]) and (c, q[0]) for c outside {q[0], q[1]}); two ranges can share one 32-word group, so the records of a
+// term exceed its distinct groups by fewer than LEV_MAX_RANGES and finalize, which merges them, still sees every group up to the cap.
+constexpr int LEV_MAX_RANGES = 2 + 2 * 254;
+constexpr int LEV_REC_SLOTS = LEV_REC_CAP + LEV_MAX_RANGES;
 struct LevTerm {
     uint8_t q[LEV_MAX_Q];
     uint8_t len;
@@ -25,6 +30,23 @@ struct LevRec {
     uint32_t base;              // first word id of the 32-word group
     uint32_t pad;
     unsigned long long codes;   // 2 bits per lane: 0 none, 1 same-first d=1, 2 same-first d=2, 3 different-first (d=1)
+};
+// Which (term, word) pairs a term's slot in a work item owns.  Every pair the filter of lev_match_kernel can accept is owned by
+// exactly one family, and each family only scans dictionary ranges where it can own pairs (DESIGN.md §3 "Term derivation").
+enum LevFamily : uint32_t {
+    LEV_F1 = 0,   // first-byte range q[0], every typo-tolerant term:              w[0] == q[0]
+    LEV_F2A = 1,  // first-byte range q[1], 2-typo terms:                          w[0] == q[1] != q[0]
+    LEV_F2B = 2,  // 2-byte ranges (c, q[1]), 2-typo terms:                        w[1] == q[1], w[0] not in {q[0], q[1]}
+    LEV_F3 = 3,   // 2-byte ranges (c, q[0]), 2-typo terms with q[0] != q[1]:      w[1] == q[0], w[0] not in {q[0], q[1]}
+    LEV_F0 = 4,   // whole dictionary, 2-typo terms with m < 2 or a zero q[0]/q[1]: w[0] != q[0]
+};
+constexpr int LEV_FAMILY_SHIFT = 29;  // term permutation entry: term index | family << LEV_FAMILY_SHIFT
+// A work item: the words [lo, lo + n) of one 256-aligned dictionary tile against the term slots perm[t_off, t_off + t_cnt)
+struct LevItem {
+    uint32_t lo;
+    uint32_t t_off;
+    uint16_t n;      // <= 256
+    uint16_t t_cnt;  // <= LEV_TERMS_PER_CTA
 };
 
 // ---- rule activations ----

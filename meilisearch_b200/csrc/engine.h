@@ -453,6 +453,10 @@ struct Engine {
     // lev buffers
     DevBuf<LevTerm> d_lev_terms;
     DevBuf<LevRec> d_lev_recs;
+    DevBuf<LevItem> d_lev_items;
+    DevBuf<uint32_t> d_lev_perm;
+    std::vector<LevItem> lev_items;  // host copies of the work list, kept to reuse their storage
+    std::vector<uint32_t> lev_perm;
     DevBuf<uint32_t> d_lev_u32;  // rec_count | one_out | n_one | two_out | n_two | status
     // vector buffers
     DevBuf<float> d_vq, d_vdist, d_vsel_dist;

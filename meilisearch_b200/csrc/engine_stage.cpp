@@ -122,6 +122,8 @@ Engine::~Engine() {
     d_sort_info.release();
     d_lev_terms.release();
     d_lev_recs.release();
+    d_lev_items.release();
+    d_lev_perm.release();
     d_lev_u32.release();
     d_vq.release();
     d_vdist.release();
@@ -157,10 +159,32 @@ void Engine::resolve_timers() {
     ev_used = 0;
 }
 
+// HostIndex::first_lo / pair_lo.  Term derivation scans the word ranges they delimit, which only holds the words of a prefix
+// when the dictionary is bytewise ascending (FST order), so anything else is refused here.
+static void build_prefix_tables(HostIndex &ix) {
+    if (ix.n_words >= (1ull << 32)) throw std::runtime_error("dictionary: more than 2^32 - 1 words");
+    for (uint64_t i = 1; i < ix.n_words; i++)
+        if (ix.cmp_word(i - 1, ix.word_ptr(i), ix.word_len(i)) >= 0)
+            throw std::runtime_error("dictionary: words are not in strictly ascending bytewise order at word " + std::to_string(i));
+    ix.first_lo.resize(257);
+    ix.pair_lo.resize(65537);
+    for (uint32_t c = 0; c < 256; c++) {
+        const uint8_t k[1] = {(uint8_t)c};
+        ix.first_lo[c] = (uint32_t)ix.lower_bound(k, 1);
+    }
+    ix.first_lo[256] = (uint32_t)ix.n_words;
+    for (uint32_t p = 0; p < 65536; p++) {
+        const uint8_t k[2] = {(uint8_t)(p >> 8), (uint8_t)p};
+        ix.pair_lo[p] = (uint32_t)ix.lower_bound(k, 2);
+    }
+    ix.pair_lo[65536] = (uint32_t)ix.n_words;
+}
+
 int Engine::stage_finish() {
     CU(cudaSetDevice(device), "cudaSetDevice");
     try {
         build_host_index(raw_dict_bytes, raw_dict_off, raw_dbs, raw_docids, hix);
+        build_prefix_tables(hix);
         build_sort_fields(raw_dbs[B200_DB_FACET_ID_F64_DOCIDS], raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], hix);
         build_geo_field(raw_dbs[B200_DB_FACET_ID_F64_DOCIDS], raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], hix);
         build_facet_search(raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], raw_dbs[B200_DB_FACET_ID_NORMALIZED_STRING_STRINGS],
@@ -336,6 +360,7 @@ int Engine::derive_batch(uint32_t n, const char *words, const uint32_t *off, con
     if (!staged) return fail(B200_ERR_STATE, "derive before b200_stage_finish");
     CU(cudaSetDevice(device), "cudaSetDevice");
     if (n == 0) return B200_OK;
+    if (n >= (1u << LEV_FAMILY_SHIFT)) return fail(B200_ERR_UNSUPPORTED, "derive: too many terms in one batch");
     std::vector<LevTerm> terms(n);
     for (uint32_t i = 0; i < n; i++) {
         uint32_t len = off[i + 1] - off[i];
@@ -349,22 +374,77 @@ int Engine::derive_batch(uint32_t n, const char *words, const uint32_t *off, con
         t.prefix = is_prefix[i] ? 1 : 0;
         if (max_typo[i] == 0) t.k_same = -1;
     }
+    // Work list (DESIGN.md §3 "Term derivation"): each term joins the groups of the dictionary ranges where its filter can accept a
+    // word, with the family that owns those pairs; a group's terms sweep each of its ranges in chunks of LEV_TERMS_PER_CTA.
+    std::vector<uint32_t> by_first[256], by_second[256], whole;
+    for (uint32_t i = 0; i < n; i++) {
+        const LevTerm &t = terms[i];
+        if (t.k_same < 0) continue;  // no typo budget: no derivations
+        by_first[t.q[0]].push_back(i | LEV_F1 << LEV_FAMILY_SHIFT);
+        if (t.k_diff < 0) continue;  // 1-typo terms keep their first byte
+        if (t.len < 2 || t.q[0] == 0 || t.q[1] == 0) {  // the filter reads w[1] = 0 for 1-byte words: sweep everything
+            whole.push_back(i | LEV_F0 << LEV_FAMILY_SHIFT);
+            continue;
+        }
+        by_second[t.q[1]].push_back(i | LEV_F2B << LEV_FAMILY_SHIFT);
+        if (t.q[1] != t.q[0]) {
+            by_first[t.q[1]].push_back(i | LEV_F2A << LEV_FAMILY_SHIFT);
+            by_second[t.q[0]].push_back(i | LEV_F3 << LEV_FAMILY_SHIFT);
+        }
+    }
+    lev_perm.clear();
+    lev_items.clear();
+    uint64_t lev_bytes = 0, lev_pairs = 0;
+    // the items of one group's term slots perm[p0, p0 + cnt) over the words [lo, hi), one per 256-word tile and term chunk
+    auto emit = [&](uint32_t p0, uint32_t cnt, uint32_t lo, uint32_t hi) {
+        for (uint32_t a = lo; a < hi;) {
+            const uint32_t b = std::min(hi, (a & ~255u) + 256);
+            for (uint32_t c = 0; c < cnt; c += LEV_TERMS_PER_CTA) {
+                const uint32_t tc = std::min(cnt - c, (uint32_t)LEV_TERMS_PER_CTA);
+                lev_items.push_back(LevItem{a, p0 + c, (uint16_t)(b - a), (uint16_t)tc});
+                lev_pairs += (uint64_t)(b - a) * tc;
+            }
+            lev_bytes += (uint64_t)((cnt + LEV_TERMS_PER_CTA - 1) / LEV_TERMS_PER_CTA) * (hix.dict_off[b] - hix.dict_off[a] + 4ull * (b - a));
+            a = b;
+        }
+    };
+    auto slots = [&](const std::vector<uint32_t> &v) {
+        lev_perm.insert(lev_perm.end(), v.begin(), v.end());
+        return (uint32_t)(lev_perm.size() - v.size());
+    };
+    for (uint32_t g = 0; g < 256; g++) {
+        if (!by_first[g].empty()) emit(slots(by_first[g]), (uint32_t)by_first[g].size(), hix.first_lo[g], hix.first_lo[g + 1]);
+        if (by_second[g].empty()) continue;
+        const uint32_t p0 = slots(by_second[g]), cnt = (uint32_t)by_second[g].size();
+        for (uint32_t c = 0; c < 256; c++)  // (g, g) holds words whose first byte is q[1] (F2B) or q[0] (F3): owned elsewhere
+            if (c != g) emit(p0, cnt, hix.pair_lo[c << 8 | g], hix.pair_hi(c, g));
+    }
+    if (!whole.empty()) emit(slots(whole), (uint32_t)whole.size(), 0, (uint32_t)hix.n_words);
+    const uint32_t n_items = (uint32_t)lev_items.size();
     CU(d_lev_terms.reserve(n), "alloc lev terms");
-    CU(d_lev_recs.reserve((size_t)n * LEV_REC_CAP), "alloc lev records");
+    CU(d_lev_items.reserve(n_items), "alloc lev work items");
+    CU(d_lev_perm.reserve(lev_perm.size()), "alloc lev term slots");
+    CU(d_lev_recs.reserve((size_t)n * LEV_REC_SLOTS), "alloc lev records");
     size_t per = 1 + 150 + 1 + 50 + 1 + 1;
     CU(d_lev_u32.reserve((size_t)n * per), "alloc lev outputs");
     uint32_t *rec_count = d_lev_u32.p, *d_one = rec_count + n, *d_n_one = d_one + (size_t)n * 150, *d_two = d_n_one + n,
              *d_n_two = d_two + (size_t)n * 50;
     int32_t *d_status = reinterpret_cast<int32_t *>(d_n_two + n);
     CU(cudaMemcpyAsync(d_lev_terms.p, terms.data(), n * sizeof(LevTerm), cudaMemcpyHostToDevice, stream), "H2D lev terms");
-    stats.h2d_bytes += n * sizeof(LevTerm);
+    if (n_items) {
+        CU(cudaMemcpyAsync(d_lev_items.p, lev_items.data(), n_items * sizeof(LevItem), cudaMemcpyHostToDevice, stream), "H2D lev items");
+        CU(cudaMemcpyAsync(d_lev_perm.p, lev_perm.data(), lev_perm.size() * 4, cudaMemcpyHostToDevice, stream), "H2D lev term slots");
+    }
+    stats.h2d_bytes += n * sizeof(LevTerm) + n_items * sizeof(LevItem) + lev_perm.size() * 4;
     stats.d2h_bytes += (size_t)n * (150 + 50 + 3) * 4;
+    stats.lev_terms += n;
+    stats.lev_items += n_items;
+    stats.lev_pairs += lev_pairs;
     size_t m0 = mark();
-    CU(launch_lev(stream, dix.dict_bytes, dix.dict_off, (uint32_t)hix.n_words, d_lev_terms.p, n, d_lev_recs.p, rec_count, d_one, d_n_one, d_two,
-                  d_n_two, d_status),
+    CU(launch_lev(stream, dix.dict_bytes, dix.dict_off, d_lev_items.p, n_items, d_lev_perm.p, d_lev_terms.p, n, d_lev_recs.p, rec_count, d_one,
+                  d_n_one, d_two, d_n_two, d_status),
        "lev kernels");
     size_t m1 = mark();
-    uint64_t lev_bytes = (uint64_t)((n + LEV_TERMS_PER_CTA - 1) / LEV_TERMS_PER_CTA) * (hix.dict_bytes.size() + 4 * hix.n_words);
     time_kernel(B200_K_LEV, m0, m1, lev_bytes);
     stats.kernel_launches += 1;
     stats.dictionary_bytes += lev_bytes;

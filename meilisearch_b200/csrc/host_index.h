@@ -110,6 +110,12 @@ struct HostIndex {
     std::vector<uint8_t> dict_bytes;
     std::vector<uint64_t> dict_off;
     uint64_t n_words = 0;
+    // prefix tables of the bytewise ascending dictionary (term derivation's work list): first_lo[c] = first word id >= "c" and
+    // pair_lo[c << 8 | g] = first word id >= "cg", so [first_lo[c], first_lo[c + 1]) holds the words starting with byte c and
+    // [pair_lo[k], pair_lo[k + 1]) (for g < 255) those starting with "cg"; the 1-byte word "c" lies in no 2-byte range
+    std::vector<uint32_t> first_lo;  // 257
+    std::vector<uint32_t> pair_lo;   // 65537
+    uint32_t pair_hi(uint32_t c, uint32_t g) const { return g < 255 ? pair_lo[(c << 8 | g) + 1] : first_lo[c + 1]; }
     // universe
     uint32_t n_docs = 0;    // max docid + 1
     uint32_t n_words64 = 0; // ceil(n_docs / 64)

@@ -22,55 +22,68 @@
 namespace b200 {
 
 // ======================================================================================== lev
-// grid.x: 256-word tiles of the dictionary; grid.y: chunks of LEV_TERMS_PER_CTA terms.
-// Two phases per group of 8 terms: (1) every thread filters its word against the 8 terms (length, first-letter rule, signature)
-// and queues the surviving (term, word) pairs in shared memory; (2) the queue is processed densely, one banded DP per thread —
-// the DP, which is the expensive part, runs on a few percent of the pairs and without divergence between matching and
+// One CTA per work item (LevItem): the words [lo, lo + n) of one 256-word dictionary tile against up to LEV_TERMS_PER_CTA term slots.
+// The host builds the items from the dictionary's first-byte and 2-byte prefix ranges, so a term only meets the words its filter
+// can accept; each slot's family (LevFamily) names the pairs it owns, so that every such pair is tested by exactly one item.
+// Two phases per group of 8 terms: (1) every thread filters its word against the 8 terms (ownership, length, first-letter rule,
+// signature) and queues the surviving (term, word) pairs in shared memory; (2) the queue is processed densely, one banded DP per
+// thread — the DP, which is the expensive part, runs on a few percent of the pairs and without divergence between matching and
 // non-matching lanes.  Match codes are collected per (term, 32-word group) and reported as ballot records.
 constexpr int LEV_TERM_GROUP = 8;
+__device__ __forceinline__ bool lev_owns(uint32_t own, uint8_t w0c, uint8_t w1c) {
+    const uint8_t q0 = (uint8_t)own, q1 = (uint8_t)(own >> 8);
+    switch (own >> 16) {
+        case LEV_F1: return w0c == q0;
+        case LEV_F2A: return w0c == q1 && q1 != q0;
+        case LEV_F2B: return w1c == q1 && w0c != q0 && w0c != q1;
+        case LEV_F3: return w1c == q0 && q0 != q1 && w0c != q0 && w0c != q1;
+        default: return w0c != q0;  // LEV_F0
+    }
+}
 __global__ void __launch_bounds__(256) lev_match_kernel(const uint8_t *__restrict__ dict_bytes, const uint32_t *__restrict__ dict_off,
-                                                        uint32_t n_words, const LevTerm *__restrict__ terms, uint32_t n_terms,
-                                                        LevRec *__restrict__ recs, uint32_t *__restrict__ rec_count) {
+                                                        const LevItem *__restrict__ items, const uint32_t *__restrict__ perm,
+                                                        const LevTerm *__restrict__ terms, LevRec *__restrict__ recs,
+                                                        uint32_t *__restrict__ rec_count) {
     __shared__ LevTerm sterms[LEV_TERMS_PER_CTA];
-    __shared__ uint32_t sterm_sig[LEV_TERMS_PER_CTA], sterm_meta[LEV_TERMS_PER_CTA];
+    __shared__ uint32_t sterm_sig[LEV_TERMS_PER_CTA], sterm_meta[LEV_TERMS_PER_CTA], sterm_own[LEV_TERMS_PER_CTA], sterm_id[LEV_TERMS_PER_CTA];
     __shared__ uint8_t sbytes[8192];
     __shared__ uint16_t s_woff[257];
     __shared__ uint32_t s_queue[LEV_TERM_GROUP * 256];  // (term << 16) | word-in-tile | (same-first << 31)
     __shared__ uint32_t s_qn;
     __shared__ unsigned long long s_codes[LEV_TERM_GROUP][8];
-    // the CTA stages its 256 dictionary words once and sweeps the term chunks blockIdx.y, blockIdx.y + gridDim.y, ... over them
-    uint32_t w0 = blockIdx.x * 256;
-    uint32_t wn = min(256u, n_words - w0);
-    uint32_t byte0 = dict_off[w0], byte1 = dict_off[w0 + wn];
-    bool in_smem = (byte1 - byte0) <= sizeof(sbytes);
+    const LevItem item = items[blockIdx.x];
+    const uint32_t tile = item.lo & ~255u, a = item.lo - tile;  // thread i <-> word tile + i; the item's words are threads [a, a + n)
+    const uint32_t nt = item.t_cnt;
+    const uint32_t byte0 = dict_off[item.lo], byte1 = dict_off[item.lo + item.n];
+    const bool in_smem = (byte1 - byte0) <= sizeof(sbytes);
     if (in_smem) {
         for (uint32_t i = threadIdx.x; i < byte1 - byte0; i += blockDim.x) sbytes[i] = dict_bytes[byte0 + i];
-        for (uint32_t i = threadIdx.x; i <= wn; i += blockDim.x) s_woff[i] = (uint16_t)(dict_off[w0 + i] - byte0);
+        for (uint32_t i = threadIdx.x; i <= item.n; i += blockDim.x) s_woff[i] = (uint16_t)(dict_off[item.lo + i] - byte0);
     }
+    if (threadIdx.x < nt) sterm_id[threadIdx.x] = perm[item.t_off + threadIdx.x];
     __syncthreads();
-    uint32_t wid = w0 + threadIdx.x;
-    bool valid = threadIdx.x < wn;
+    {
+        constexpr uint32_t W = sizeof(LevTerm) / 4;
+        uint32_t *dst = reinterpret_cast<uint32_t *>(sterms);
+        for (uint32_t i = threadIdx.x; i < nt * W; i += blockDim.x) {
+            const uint32_t t = sterm_id[i / W] & ((1u << LEV_FAMILY_SHIFT) - 1);
+            dst[i] = reinterpret_cast<const uint32_t *>(terms + t)[i % W];
+        }
+    }
+    const uint32_t wid = tile + threadIdx.x;
+    const bool valid = threadIdx.x >= a && threadIdx.x < a + item.n;
     uint32_t off = valid ? dict_off[wid] : byte0;
     int n = valid ? (int)(dict_off[wid + 1] - off) : 0;
     const uint8_t *w = in_smem ? (sbytes + (off - byte0)) : (dict_bytes + off);
     uint8_t w0c = n > 0 ? w[0] : 0, w1c = n > 1 ? w[1] : 0;
-    const uint32_t wsig = char_signature(w, n);
-    const uint32_t n_chunks = (n_terms + LEV_TERMS_PER_CTA - 1) / LEV_TERMS_PER_CTA;
-    for (uint32_t chunk = blockIdx.y; chunk < n_chunks; chunk += gridDim.y) {
-    const uint32_t t0 = chunk * LEV_TERMS_PER_CTA;
-    const uint32_t nt = min((uint32_t)LEV_TERMS_PER_CTA, n_terms - t0);
-    __syncthreads();  // the previous chunk's terms are no longer read
-    {
-        const uint32_t *src = reinterpret_cast<const uint32_t *>(terms + t0);
-        uint32_t *dst = reinterpret_cast<uint32_t *>(sterms);
-        for (uint32_t i = threadIdx.x; i < nt * sizeof(LevTerm) / 4; i += blockDim.x) dst[i] = src[i];
-    }
     __syncthreads();
+    const uint32_t wsig = char_signature(w, n);
     if (threadIdx.x < nt) {
         const LevTerm &T = sterms[threadIdx.x];
         sterm_sig[threadIdx.x] = char_signature(T.q, T.len);
         sterm_meta[threadIdx.x] = (uint32_t)T.len | ((uint32_t)(T.k_same + 1) << 8) | ((uint32_t)(T.k_diff + 1) << 12) |
                                   ((uint32_t)(T.prefix ? 1 : 0) << 16) | ((uint32_t)T.q[0] << 24);
+        sterm_own[threadIdx.x] = (uint32_t)T.q[0] | ((uint32_t)T.q[1] << 8) | ((sterm_id[threadIdx.x] >> LEV_FAMILY_SHIFT) << 16);
     }
     for (uint32_t tg = 0; tg < nt; tg += LEV_TERM_GROUP) {
         const uint32_t ng = min((uint32_t)LEV_TERM_GROUP, nt - tg);
@@ -84,6 +97,7 @@ __global__ void __launch_bounds__(256) lev_match_kernel(const uint8_t *__restric
                 const uint32_t meta = sterm_meta[tg + t];  // len | (k_same+1) << 8 | (k_diff+1) << 12 | prefix << 16 | q0 << 24
                 const int kmax = (int)((meta >> 8) & 15) - 1;
                 if (__popc(tsig & ~wsig) > kmax) continue;
+                if (!lev_owns(sterm_own[tg + t], w0c, w1c)) continue;
                 const bool prefix = (meta >> 16) & 1;
                 const bool sf = (uint8_t)(meta >> 24) == w0c;
                 const int k = sf ? kmax : (int)((meta >> 12) & 15) - 1;
@@ -111,12 +125,12 @@ __global__ void __launch_bounds__(256) lev_match_kernel(const uint8_t *__restric
             const uint8_t *ww;
             int wl;
             if (in_smem) {
-                ww = sbytes + s_woff[wi];
-                wl = (int)s_woff[wi + 1] - (int)s_woff[wi];
+                ww = sbytes + s_woff[wi - a];
+                wl = (int)s_woff[wi - a + 1] - (int)s_woff[wi - a];
             } else {
-                uint32_t o = dict_off[w0 + wi];
+                uint32_t o = dict_off[tile + wi];
                 ww = dict_bytes + o;
-                wl = (int)(dict_off[w0 + wi + 1] - o);
+                wl = (int)(dict_off[tile + wi + 1] - o);
             }
             int d = banded_osa(T.q, T.len, ww, wl, k, T.prefix != 0);
             if (d <= k && d > 0) {
@@ -130,18 +144,18 @@ __global__ void __launch_bounds__(256) lev_match_kernel(const uint8_t *__restric
             const uint32_t t = threadIdx.x >> 3, g = threadIdx.x & 7;
             const unsigned long long codes = s_codes[t][g];
             if (codes) {
-                uint32_t slot = atomicAdd(&rec_count[t0 + tg + t], 1u);
-                if (slot < LEV_REC_CAP) {
+                const uint32_t term = sterm_id[tg + t] & ((1u << LEV_FAMILY_SHIFT) - 1);
+                uint32_t slot = atomicAdd(&rec_count[term], 1u);
+                if (slot < LEV_REC_SLOTS) {
                     LevRec r;
-                    r.base = w0 + g * 32;
+                    r.base = tile + g * 32;
                     r.pad = 0;
                     r.codes = codes;
-                    recs[(size_t)(t0 + tg + t) * LEV_REC_CAP + slot] = r;
+                    recs[(size_t)term * LEV_REC_SLOTS + slot] = r;
                 }
             }
         }
         __syncthreads();
-    }
     }
 }
 
@@ -153,12 +167,9 @@ __global__ void lev_finalize_kernel(LevRec *__restrict__ recs, const uint32_t *_
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n_terms) return;
     uint32_t cnt = rec_count[t];
-    if (cnt > LEV_REC_CAP) {
-        status[t] = -5;
-        cnt = LEV_REC_CAP;
-    } else
-        status[t] = 0;
-    LevRec *r = recs + (size_t)t * LEV_REC_CAP;
+    status[t] = cnt > LEV_REC_SLOTS ? -5 : 0;
+    cnt = min(cnt, (uint32_t)LEV_REC_SLOTS);
+    LevRec *r = recs + (size_t)t * LEV_REC_SLOTS;
     for (uint32_t i = 1; i < cnt; i++) {  // insertion sort by base
         LevRec x = r[i];
         uint32_t j = i;
@@ -167,6 +178,19 @@ __global__ void lev_finalize_kernel(LevRec *__restrict__ recs, const uint32_t *_
             j--;
         }
         r[j] = x;
+    }
+    // items that split a 32-word group report it separately, each with the codes of its own words: merge them
+    uint32_t u = 0;
+    for (uint32_t i = 0; i < cnt; i++) {
+        if (u > 0 && r[u - 1].base == r[i].base)
+            r[u - 1].codes |= r[i].codes;
+        else
+            r[u++] = r[i];
+    }
+    cnt = u;
+    if (cnt > LEV_REC_CAP) {
+        status[t] = -5;
+        cnt = LEV_REC_CAP;
     }
     bool two_budget = terms[t].k_same >= 2;
     uint32_t c1 = 0, c2 = 0;
@@ -1409,14 +1433,12 @@ cudaError_t launch_shard_merge(cudaStream_t s, const uint32_t *g_ids, const floa
         if (e_ != cudaSuccess) return e_; \
     } while (0)
 
-cudaError_t launch_lev(cudaStream_t s, const uint8_t *dict_bytes, const uint32_t *dict_off, uint32_t n_words, const LevTerm *terms,
-                       uint32_t n_terms, LevRec *recs, uint32_t *rec_count, uint32_t *one_out, uint32_t *n_one, uint32_t *two_out,
+cudaError_t launch_lev(cudaStream_t s, const uint8_t *dict_bytes, const uint32_t *dict_off, const LevItem *items, uint32_t n_items,
+                       const uint32_t *perm, const LevTerm *terms, uint32_t n_terms, LevRec *recs, uint32_t *rec_count, uint32_t *one_out, uint32_t *n_one, uint32_t *two_out,
                        uint32_t *n_two, int32_t *status) {
-    if (n_terms == 0 || n_words == 0) return cudaSuccess;
+    if (n_terms == 0) return cudaSuccess;
     CK(cudaMemsetAsync(rec_count, 0, sizeof(uint32_t) * n_terms, s));
-    const uint32_t n_chunks = (n_terms + LEV_TERMS_PER_CTA - 1) / LEV_TERMS_PER_CTA;
-    dim3 grid((n_words + 255) / 256, n_chunks < 8 ? n_chunks : 8);  // every CTA sweeps n_chunks / 8 term chunks over its word tile
-    lev_match_kernel<<<grid, 256, 0, s>>>(dict_bytes, dict_off, n_words, terms, n_terms, recs, rec_count);
+    if (n_items) lev_match_kernel<<<n_items, 256, 0, s>>>(dict_bytes, dict_off, items, perm, terms, recs, rec_count);
     lev_finalize_kernel<<<(n_terms + 63) / 64, 64, 0, s>>>(recs, rec_count, terms, n_terms, one_out, n_one, two_out, n_two, status);
     return cudaGetLastError();
 }
