@@ -2541,9 +2541,10 @@ struct KeywordBatch {
         if (const char *env = getenv("B200_DRIVERS")) n_drivers = (unsigned)std::max(1, std::min((int)Engine::MAX_DRIVERS, atoi(env)));
         if (const char *env = getenv("B200_LANES_PER_DRIVER")) lanes_per_driver = (unsigned)std::max(1, atoi(env));
         if (getenv("B200_SINGLE_LANE")) n_drivers = lanes_per_driver = 1;
-        n_lanes = std::min<unsigned>(Engine::MAX_LANES, n_drivers * lanes_per_driver);
+        // every lane that is given queries belongs to a driver: drive() and drive_waves() run lanes [0, n_drivers * lanes_per_driver)
+        lanes_per_driver = std::min(lanes_per_driver, Engine::MAX_LANES / n_drivers);
+        n_lanes = n_drivers * lanes_per_driver;
         if (NQ < n_lanes) n_lanes = n_drivers = lanes_per_driver = 1;
-        lanes_per_driver = n_lanes / n_drivers;
         {
             unsigned per_driver = std::max(1u, host_threads() / n_drivers);
             for (unsigned dr = 0; dr < n_drivers; dr++) {

@@ -318,9 +318,12 @@ def test_large_universe_matches_oracle(mb):
 
 def test_union_postings_matches_decoded_lists(mb, synth):
     """S2 (b200_union_postings): OR of posting lists AND universe, against the CBO values decoded by the oracle's codec."""
+    check_union_postings(mb.Index(synth), synth)
+
+
+def check_union_postings(ix, synth):
     from oracle.pyoracle import cbo_decode
 
-    ix = mb.Index(synth)
     rng = np.random.default_rng(3)
     n_words = (synth.n_docs + 63) // 64
     for db in (0, 4, 5):  # word_docids, word_pair_proximity_docids, word_position_docids
