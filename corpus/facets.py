@@ -5,7 +5,10 @@ value: FacetGroupValueCodec = u8 size | CBO roaring (heed_codec/facet/mod.rs).  
 group FACET_GROUP_SIZE entries of the level below (left bound = the first one's) as the reference's incremental indexer does, so
 that readers which must ignore them see them.  JSON documents go through milli's extraction rules: arrays are flattened, `null`,
 objects and the empty string get no facet, booleans become the strings "true" / "false", strings are normalised (lib.rs:442).
-`_geo` objects become the number facets `_geo.lat` / `_geo.lng` (update/new/extract/faceted/facet_document.rs:82-99)."""
+`_geo` objects become the number facets `_geo.lat` / `_geo.lng` (update/new/extract/faceted/facet_document.rs:82-99).
+build_presence() adds facet_id_{exists,is_null,is_empty}_docids (key u16 BE fid, value CBO) as extract_facets.rs writes them: a field
+exists in a document for any value, `null`, `[]`, `{}` and non-empty objects included; it is null for a top-level `null` and empty for
+a top-level `""`, `[]` or `{}`.  add_document walks a whole document as milli does, nested objects included (dotted field names)."""
 from __future__ import annotations
 
 import struct
@@ -89,6 +92,9 @@ class FacetImage:
         # (fid, docid, normalised str) -> original string, what field_id_docid_facet_strings holds.  A document can give one normalised
         # value several originals ("Blue" and "blue " in one array); the first one it gives is kept.
         self.originals = {}
+        # fid -> docids: documents holding the field with a value that gives no number or string facet (exists), and with a
+        # top-level null / "" [] {} (is_null / is_empty); documents with a facet value exist without being listed here
+        self.present, self.null, self.empty = {}, {}, {}
 
     def fid(self, name):
         if name not in self.fields:
@@ -106,9 +112,10 @@ class FacetImage:
         else:
             self.numbers.setdefault(f, {}).setdefault(float(value), []).append(docid)
 
-    def add_json(self, docid, name, value):
+    def add_json(self, docid, name, value, top=True):
         """a JSON field value through milli's facet extraction: arrays flattened; null / objects / "" give nothing; `_geo`
-        ({"lat": .., "lng": ..}, numbers or numeric strings) gives the number facets `_geo.lat` / `_geo.lng`"""
+        ({"lat": .., "lng": ..}, numbers or numeric strings) gives the number facets `_geo.lat` / `_geo.lng`.  A top-level null, "",
+        [] or {} is recorded for build_presence, and so is a document holding the field at all."""
         if name == "_geo":
             if value is None:
                 return
@@ -116,16 +123,85 @@ class FacetImage:
             self.add_facet(docid, "_geo.lat", lat)
             self.add_facet(docid, "_geo.lng", lng)
             return
-        self.fid(name)
+        f = self.fid(name)
+        if top:  # extract_facets.rs:309-313: every value the field holds, objects and arrays included, makes it exist
+            self.present.setdefault(f, set()).add(docid)
+            if value is None:
+                self.null.setdefault(f, set()).add(docid)
+            elif value in ("", [], {}):
+                self.empty.setdefault(f, set()).add(docid)
         if isinstance(value, list):
             for v in value:
-                self.add_json(docid, name, v)
+                self.add_json(docid, name, v, top=False)
         elif isinstance(value, bool):
             self.add_facet(docid, name, "true" if value else "false")
         elif isinstance(value, (int, float)):
             self.add_facet(docid, name, value)
         elif isinstance(value, str):
             self.add_facet(docid, name, value)
+
+    def _extract_field(self, docid, name, on_base, value):
+        """extract_facets.rs facet_fn_with_options (:300-410) for one value the walk reaches"""
+        f = self.fid(name)
+        self.present.setdefault(f, set()).add(docid)
+        if isinstance(value, bool):
+            v = "true" if value else "false"
+            self.strings.setdefault(f, {}).setdefault(v, []).append(docid)
+            self.originals.setdefault((f, docid, v), v)
+        elif isinstance(value, (int, float)):
+            self.numbers.setdefault(f, {}).setdefault(float(value), []).append(docid)
+        elif isinstance(value, str) and value:
+            v = normalize_facet(value)
+            self.strings.setdefault(f, {}).setdefault(v, []).append(docid)
+            self.originals.setdefault((f, docid, v), value)
+        elif on_base and value is None:
+            self.null.setdefault(f, set()).add(docid)
+        elif on_base and value in ("", [], {}):
+            self.empty.setdefault(f, set()).add(docid)
+
+    def _seek_object(self, docid, obj, base, on_base, keep):
+        """perm_json_p::seek_leaf_values_in_object (update/new/extract/mod.rs:34-66)"""
+        if not obj:
+            self._visit(docid, base, on_base, {}, keep)
+        for k, v in obj.items():
+            key = f"{base}.{k}" if base else k
+            self._visit(docid, key, True, v, keep)
+            if isinstance(v, dict):
+                self._seek_object(docid, v, key, True, keep)
+            elif isinstance(v, list):
+                self._seek_array(docid, v, key, True, keep)
+
+    def _seek_array(self, docid, arr, base, on_base, keep):
+        """perm_json_p::seek_leaf_values_in_array (update/new/extract/mod.rs:68-91)"""
+        if not arr:
+            self._visit(docid, base, on_base, [], keep)
+        for v in arr:
+            if isinstance(v, dict):
+                self._seek_object(docid, v, base, False, keep)
+            elif isinstance(v, list):
+                self._seek_array(docid, v, base, False, keep)
+            else:
+                self._visit(docid, base, False, v, keep)
+
+    def _visit(self, docid, name, on_base, value, keep):
+        if keep(name):
+            self._extract_field(docid, name, on_base, value)
+
+    def add_document(self, docid, doc, filterable):
+        """a whole JSON document through milli's facet extraction (facet_document.rs:20-99): every field matching a name in
+        `filterable`, or nested under one (`opt1.opt2` under `opt1`), is extracted at every value the walk reaches; an object or
+        array field is first walked, then extracted itself; `_geo` becomes `_geo.lat` / `_geo.lng`"""
+        keep = lambda name: any(name == p or name.startswith(p + ".") for p in filterable)  # noqa: E731
+        for name, value in doc.items():
+            if name == "_geo":
+                if "_geo" in filterable:
+                    self.add_json(docid, "_geo", value)
+                continue
+            if isinstance(value, dict):
+                self._seek_object(docid, value, name, True, keep)
+            elif isinstance(value, list):
+                self._seek_array(docid, value, name, True, keep)
+            self._visit(docid, name, True, value, keep)
 
     def add_synthetic(self, n_docs, seed=0x50A7):
         """seeded facet fields: `price` (numbers with many duplicates, ~10 % missing), `brand` (Zipf-distributed strings), `tags`
@@ -199,6 +275,18 @@ class FacetImage:
         self.f64_db = _db(self._entries(self.numbers, lambda v: ordered_f64(v)))
         self.string_db = _db(self._entries(self.strings, lambda v: v.encode()))
         return self.f64_db, self.string_db
+
+    def build_presence(self):
+        """-> (facet_id_exists_docids, facet_id_is_null_docids, facet_id_is_empty_docids) as DbImage, keys in LMDB order; also kept as
+        self.exists_db / self.null_db / self.empty_db, which Index.stage stages when present"""
+        exists = {f: set(d) for f, d in self.present.items()}
+        for tab in (self.numbers, self.strings):
+            for f, vals in tab.items():
+                for docs in vals.values():
+                    exists.setdefault(f, set()).update(int(x) for x in docs)
+        dbs = [_db(sorted((struct.pack(">H", f), cbo_encode(sorted(d))) for f, d in tab.items() if d)) for tab in (exists, self.null, self.empty)]
+        self.exists_db, self.null_db, self.empty_db = dbs
+        return tuple(dbs)
 
     def build_search(self):
         """-> (facet_id_normalized_string_strings, field_id_docid_facet_strings) as DbImage, keys in LMDB order: per string field

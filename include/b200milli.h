@@ -65,7 +65,13 @@ enum b200_db {
      * (heed_codec/facet/field_doc_id_facet_codec.rs, index.rs:181-188). */
     B200_DB_FACET_ID_NORMALIZED_STRING_STRINGS = 12,
     B200_DB_FIELD_ID_DOCID_FACET_STRINGS = 13,
-    B200_DB_COUNT = 14
+    /* facet databases read by the EXISTS / IS NULL / IS EMPTY filters (Index::{exists,null,empty}_faceted_documents_ids).  Key: u16
+     * BE fid; value: CBO bytes.  An index staged without one of them searches as before; a filter program with a leaf that reads a
+     * database that was not staged fails its query with B200_ERR_INVALID. */
+    B200_DB_FACET_ID_EXISTS_DOCIDS = 14,
+    B200_DB_FACET_ID_IS_NULL_DOCIDS = 15,
+    B200_DB_FACET_ID_IS_EMPTY_DOCIDS = 16,
+    B200_DB_COUNT = 17
 };
 /* Replaces Index::words_fst (index.rs:1238): the FST enumerated once on the host into its sorted word list. */
 int b200_stage_dictionary(b200_index *, const uint8_t *word_bytes, const uint64_t *word_offsets, uint64_t n_words);
@@ -174,6 +180,57 @@ int b200_nns_batch_sharded(b200_index *, const float *queries, uint32_t n_q, uin
  * Queries arrive tokenised (charabia stays on the host): tokens of query i are
  * [token_begin[i], token_begin[i+1]); kind: 0 Word, 1 StopWord, 2 Separator(Soft), 3 Separator(Hard). */
 enum b200_tms { B200_TMS_LAST = 0, B200_TMS_ALL = 1, B200_TMS_FREQUENCY = 2 };
+
+/* Filter programs: the parsed FilterCondition tree of IndexFilter::inner_evaluate (search/facet/filter/index_filter.rs:332-696),
+ * as a Rust shim gets it from filter-parser, after the caller's not-filterable check of `evaluate` (:43-73).  Program i is the nodes
+ * [begin[i], begin[i + 1]) in pre-order (an empty range: no filter).  AND / OR take the next `n` subtrees as their children, in
+ * order; NOT the next one.  Value strings arrive normalize_facet'd; a value's number is what parse_finite_float gives, NaN when it
+ * does not parse.  Semantics (bitmaps, `docs` = documents_ids):
+ *   RANGE(fid, lo, hi, values [value, value + 2)): the level-0 keys of facet_id_f64_docids between the numbers of the two values
+ *     (only when has_number: for `TO` both ends parse, for `>`, `>=`, `<`, `<=` the one given), in OrderedF64 key order, plus the
+ *     keys of facet_id_string_docids between the two strings in byte order (ValueBounds::new); lo / hi are b200_bound kinds, the
+ *     same for both; an inverted interval is empty.
+ *   EQUAL(fid, value): the string key's docids OR the number key's docids when the number parses (evaluate_equal).  NOT_EQUAL:
+ *     docs - EQUAL.  IN(fid, values [value, value + n)): the union of the EQUALs.
+ *   EXISTS / IS_NULL / IS_EMPTY(fid): the field's entry in B200_DB_FACET_ID_{EXISTS,IS_NULL,IS_EMPTY}_DOCIDS.
+ *   GEO_RADIUS / GEO_BBOX: args as b200_query_batch::geo_filter_args; a GEO_BBOX is the range conditions on `_geo.lat` /
+ *     `_geo.lng` it stands for, so it intersects with its hint like RANGE.  EMPTY: nothing (a field absent from the fields map or
+ *     matching no filterable rule).  DENIED(fid): the field's FilterableAttributesFeatures forbid the operator (the caller keeps the
+ *     message).  AND of zero children: nothing.  NOT x: docs - x.
+ * A value leaf on a fid without facet values matches nothing.  The reference raises a leaf's error only when evaluation reaches it:
+ * AND stops at an empty running bitmap and passes it as the universe hint of its next child; RANGE, GEO_BBOX and NOT intersect with
+ * their hint, the other leaves ignore it; a node whose hint is empty is not evaluated.  The library reproduces that reach exactly: a
+ * DENIED leaf, or a geo leaf with bad arguments or on an index without b200_stage_geo_fields (`_geo` not filterable), fails its
+ * query with B200_ERR_INVALID and the reference's message only when reached, the first in pre-order winning.  Per query, whatever is
+ * reached: an UNSUPPORTED node (CONTAINS, STARTS WITH, _geoPolygon, _geojson, the `resolution` argument, _vectors, the `_shard`
+ * field) or nesting deeper than B200_MAX_FILTER_DEPTH nodes (milli's MAX_FILTER_DEPTH, search/facet/filter/mod.rs, the bound
+ * IndexFilter::evaluate walks the tree with) is B200_ERR_UNSUPPORTED; EXISTS / IS_NULL / IS_EMPTY without their staged database, an
+ * unknown op or a tree that does not fit its node range is B200_ERR_INVALID. */
+#define B200_MAX_FILTER_DEPTH 2000
+enum b200_filter_op { B200_F_AND = 0, B200_F_OR = 1, B200_F_NOT = 2, B200_F_RANGE = 3, B200_F_EQUAL = 4, B200_F_NOT_EQUAL = 5, B200_F_IN = 6,
+                      B200_F_EXISTS = 7, B200_F_IS_NULL = 8, B200_F_IS_EMPTY = 9, B200_F_GEO_RADIUS = 10, B200_F_GEO_BBOX = 11,
+                      B200_F_EMPTY = 12, B200_F_DENIED = 13, B200_F_UNSUPPORTED = 14 };
+enum b200_bound { B200_B_INCLUDED = 0, B200_B_EXCLUDED = 1, B200_B_UNBOUNDED = 2 };
+typedef struct {
+    uint8_t op;          /* b200_filter_op */
+    uint8_t lo, hi;      /* RANGE: b200_bound of each end */
+    uint8_t has_number;  /* RANGE: the number bounds exist */
+    uint16_t fid;        /* the field's id in the facet databases */
+    uint16_t pad;
+    uint32_t n;          /* AND / OR: children; IN: values */
+    uint32_t value;      /* RANGE, EQUAL, NOT_EQUAL, IN: the first value */
+    double args[4];      /* GEO_RADIUS / GEO_BBOX */
+} b200_filter_node;
+typedef struct {
+    uint32_t n;                      /* programs */
+    const uint32_t *begin;           /* n + 1 node offsets */
+    const b200_filter_node *nodes;
+    uint32_t n_values;
+    const uint32_t *value_off;       /* n_values + 1: value v is value_bytes[value_off[v] .. value_off[v + 1]) */
+    const char *value_bytes;
+    const double *value_num;         /* value v's number, NaN = none */
+} b200_filter_programs;
+
 typedef struct {
     uint32_t n_queries;
     const uint32_t *token_begin;  /* n_queries + 1 */
@@ -278,6 +335,11 @@ typedef struct {
     const char *facet_query_bytes;
     const uint8_t *facet_search_flags;
     uint32_t facet_search_max;
+    /* The `filter` search parameter (NULL = none): program i filters query i (filter->n == n_queries).  The query's filtered universe
+     * is documents_ids AND universes[i] AND its geo_filter_* clauses AND its program; every mode and the facet outputs take it as
+     * they take `universes`.  Queries with the same universe pointer, geo clauses and program bytes share one device bitmap.  Errors
+     * (see b200_filter_programs) fail the query alone; b200_results::filter_error_leaf names the failing leaf. */
+    const b200_filter_programs *filter;
 } b200_query_batch;
 #define B200_MAX_SCORES 12
 /* score kinds: ScoreDetails variants (score_details.rs:9-32) */
@@ -335,6 +397,9 @@ typedef struct {                  /* SearchResult (search/mod.rs:526-535), flatt
     uint64_t *fs_count;
     uint32_t *fs_docid;
     uint8_t *fs_fallback;
+    /* n_queries (may be NULL): the node index, relative to the query's first node, of the filter node whose error failed the query
+     * (a reached failing leaf, an unsupported node, a leaf without its staged database), -1 when no node's error did */
+    int32_t *filter_error_leaf;
 } b200_results;
 int b200_search_batch(b200_index *, const b200_query_batch *, b200_results *);
 
@@ -343,6 +408,13 @@ int b200_search_batch(b200_index *, const b200_query_batch *, b200_results *);
  * out[i * out_words ..] (out_words >= ceil((max docid + 1) / 64); words past the document range are zero).  status[i]: 0 or
  * B200_ERR_INVALID with the reference's message (its bitmap is then empty).  The same kernels as the search batch. */
 int b200_geo_filter_batch(b200_index *, uint32_t n, const uint8_t *kind, const double *args, uint64_t *out, uint64_t out_words, int32_t *status);
+
+/* Replaces IndexFilter::evaluate after its not-filterable check (index_filter.rs:43-73) for callers that filter outside a search
+ * (facet distribution with a filter, document fetch or delete by filter): program i (b200_query_batch::filter semantics) becomes the
+ * dense bitmap out[i * out_words ..] (out_words >= ceil((max docid + 1) / 64); words past the document range are zero).  status[i]:
+ * 0 or the program's error (its bitmap is then empty); error_leaf[i] (may be NULL) as b200_results::filter_error_leaf.  The same
+ * kernels as the search batch. */
+int b200_filter_batch(b200_index *, const b200_filter_programs *programs, uint64_t *out, uint64_t out_words, int32_t *status, int32_t *error_leaf);
 
 /* Replaces FacetDistribution::execute and compute_stats (search/facet/facet_distribution.rs:110-337) for callers that hold the
  * candidates themselves (semantic and hybrid searches, the S1 seam, federated search): candidate set i is the host bitmap
@@ -414,7 +486,7 @@ void b200_rule_end(b200_rule *);
 /* kernel classes for the per-kernel accounting below */
 enum b200_kernel { B200_K_LEV = 0, B200_K_COMPACT = 1, B200_K_PAIR_PROBE = 2, B200_K_SCATTER = 3, B200_K_EVAL_PATHS = 4, B200_K_EMIT = 5,
                    B200_K_VEC_DIST = 6, B200_K_TOPK = 7, B200_K_VEC_GEMM = 8, B200_K_VEC_MERGE = 9, B200_K_SORT = 10, B200_K_GEO = 11,
-                   B200_K_GEO_FILTER = 12, B200_K_FACET = 13, B200_K_FACET_SEARCH = 14, B200_K_COUNT = 15 };
+                   B200_K_GEO_FILTER = 12, B200_K_FACET = 13, B200_K_FACET_SEARCH = 14, B200_K_FILTER = 15, B200_K_COUNT = 16 };
 typedef struct {
     uint64_t kernel_launches;     /* kernels launched by the library since the last reset */
     uint64_t device_steps;        /* host<->device round trips since the last reset */

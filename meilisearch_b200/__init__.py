@@ -14,6 +14,7 @@ import subprocess
 
 import numpy as np
 
+from .filter import parse_filter, preorder  # noqa: F401
 from .tokenizer import TokenBatch, tokenize  # noqa: F401
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -26,6 +27,7 @@ SCORE_KINDS = ["words", "typo", "proximity", "fid", "position", "exactAttribute"
 GEO_STRATEGIES = {"dynamic": 0, "iterative": 1, "rtree": 2}  # GeoSortStrategy::Dynamic / AlwaysIterative / AlwaysRtree
 DB_FACET_F64, DB_FACET_STRING = 10, 11
 DB_FACET_NORMALIZED, DB_FACET_ORIGINALS = 12, 13  # facet_id_normalized_string_strings, field_id_docid_facet_strings
+DB_FACET_EXISTS, DB_FACET_IS_NULL, DB_FACET_IS_EMPTY = 14, 15, 16  # facet_id_{exists,is_null,is_empty}_docids
 NO_FIELD = 0xFFFF  # a sort field absent from the fields map
 ERRORS = {-1: "NO_DEVICE", -2: "CUDA", -3: "INVALID", -4: "UNSUPPORTED", -5: "CAPACITY", -6: "STATE"}
 
@@ -54,7 +56,7 @@ class _Batch(C.Structure):
                 ("geo_filter_not", C.c_void_p), ("geo_filter_args", C.c_void_p), ("facet_begin", C.c_void_p), ("facet_fid", C.c_void_p),
                 ("facet_order", C.c_void_p), ("facet_max_values", C.c_uint32), ("facet_cap", C.c_uint32), ("facet_search_fid", C.c_void_p),
                 ("facet_query_kind", C.c_void_p), ("facet_query_off", C.c_void_p), ("facet_query_bytes", C.c_void_p),
-                ("facet_search_flags", C.c_void_p), ("facet_search_max", C.c_uint32)]
+                ("facet_search_flags", C.c_void_p), ("facet_search_max", C.c_uint32), ("filter", C.c_void_p)]
 
 
 class _Results(C.Structure):
@@ -63,19 +65,24 @@ class _Results(C.Structure):
                [("candidates_words", C.c_uint64)] + \
                [(n, C.c_void_p) for n in ("facet_n_num", "facet_n_str", "facet_key", "facet_count", "facet_docid", "facet_has_stats", "facet_min",
                                           "facet_max")] + \
-               [(n, C.c_void_p) for n in ("fs_n", "fs_key", "fs_count", "fs_docid", "fs_fallback")]
+               [(n, C.c_void_p) for n in ("fs_n", "fs_key", "fs_count", "fs_docid", "fs_fallback", "filter_error_leaf")]
+
+
+class _FilterPrograms(C.Structure):
+    _fields_ = [("n", C.c_uint32), ("begin", C.c_void_p), ("nodes", C.c_void_p), ("n_values", C.c_uint32), ("value_off", C.c_void_p),
+                ("value_bytes", C.c_void_p), ("value_num", C.c_void_p)]
 
 
 class _Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("device_steps", C.c_uint64), ("posting_bytes", C.c_uint64), ("matrix_bytes", C.c_uint64),
-                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 15),
-                ("kernel_count", C.c_uint64 * 15), ("kernel_bytes", C.c_uint64 * 15), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
+                ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 16),
+                ("kernel_count", C.c_uint64 * 16), ("kernel_bytes", C.c_uint64 * 16), ("device_ms", C.c_double), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("host_ms", C.c_double * 8),
                 ("hbm_bytes_staged", C.c_uint64), ("deferred", C.c_uint64), ("arena_peak_bytes", C.c_uint64),
                 ("eval_class_launches", C.c_uint64 * 9), ("eval_class_tiles", C.c_uint64 * 9),
                 ("lev_terms", C.c_uint64), ("lev_items", C.c_uint64), ("lev_pairs", C.c_uint64)]
 
 
-KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort", "geo", "geo_filter", "facet", "facet_search"]
+KERNELS = ["lev_match", "act_compact", "pair_probe", "scatter", "eval_paths", "emit", "vec_dist", "topk_select", "vec_gemm_topk", "vec_merge", "sort", "geo", "geo_filter", "facet", "facet_search", "filter"]
 
 
 def build_library(force=False):
@@ -120,6 +127,7 @@ def load_library():
         l.b200_comm_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         l.b200_search_batch.argtypes = [C.c_void_p, C.POINTER(_Batch), C.POINTER(_Results)]
         l.b200_geo_filter_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+        l.b200_filter_batch.argtypes = [C.c_void_p, C.POINTER(_FilterPrograms), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
         l.b200_facet_distribution_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
                                                     C.c_uint32] + [C.c_void_p] * 9
         l.b200_facet_search_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64] + [C.c_void_p] * 5 + [C.c_uint32, C.c_uint32] + \
@@ -138,7 +146,7 @@ def load_library():
 
 SYMBOLS = ["b200_open", "b200_close", "b200_last_error", "b200_open_error", "b200_stage_dictionary", "b200_stage_db",
            "b200_stage_documents_ids", "b200_stage_settings", "b200_stage_synonyms", "b200_stage_geo_fields", "b200_stage_finish", "b200_stage_embeddings", "b200_stage_embeddings_f16", "b200_stage_distribution",
-           "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_geo_filter_batch", "b200_facet_distribution_batch", "b200_facet_search_batch", "b200_graph_from_tokens",
+           "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_geo_filter_batch", "b200_filter_batch", "b200_facet_distribution_batch", "b200_facet_search_batch", "b200_graph_from_tokens",
            "b200_graph_free", "b200_rule_start", "b200_rule_next", "b200_rule_end", "b200_get_stats", "b200_reset_stats"]
 
 
@@ -182,6 +190,102 @@ def parse_geo_filter(clause):
 
 def _p(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
+
+
+F_AND, F_OR, F_NOT, F_RANGE, F_EQUAL, F_NOT_EQUAL, F_IN, F_EXISTS, F_IS_NULL, F_IS_EMPTY, F_GEO_RADIUS, F_GEO_BBOX, F_EMPTY, F_DENIED, \
+    F_UNSUPPORTED = range(15)
+B_INCLUDED, B_EXCLUDED, B_UNBOUNDED = 0, 1, 2
+FILTER_NODE = np.dtype({"names": ["op", "lo", "hi", "has_number", "fid", "pad", "n", "value", "args"],
+                        "formats": ["u1", "u1", "u1", "u1", "<u2", "<u2", "<u4", "<u4", ("<f8", 4)],
+                        "offsets": [0, 1, 2, 3, 4, 6, 8, 12, 16], "itemsize": 48})
+# the FilterableAttributesFeatures check each operator makes (index_filter.rs:94-125)
+OP_FEATURE = {">": "comparison", ">=": "comparison", "<": "comparison", "<=": "comparison", "TO": "comparison", "=": "equality",
+              "!=": "equality", "IN": "equality", "EXISTS": "exists", "NULL": "null", "EMPTY": "empty"}
+_RANGE = {">": (B_EXCLUDED, B_UNBOUNDED), ">=": (B_INCLUDED, B_UNBOUNDED), "<": (B_UNBOUNDED, B_EXCLUDED), "<=": (B_UNBOUNDED, B_INCLUDED),
+          "TO": (B_INCLUDED, B_INCLUDED)}
+
+
+class _Programs:
+    """the arrays of a b200_filter_programs and the struct pointing at them"""
+
+    def __init__(self, nodes, begin, values):
+        from corpus.facets import normalize_facet
+        from .filter import parse_finite_float
+
+        self.nodes = np.asarray(nodes if nodes else [np.zeros((), FILTER_NODE)], FILTER_NODE)
+        self.begin = np.asarray(begin, np.uint32)
+        enc = [normalize_facet(v).encode() for v in values]
+        self.off = np.zeros(len(values) + 1, np.uint32)
+        self.off[1:] = np.cumsum([len(e) for e in enc]) if enc else []
+        self.bytes = np.frombuffer(b"".join(enc) + b"\0", np.uint8).copy()
+        nums = [parse_finite_float(v) for v in values]
+        self.num = np.asarray([np.nan if x is None else x for x in nums] or [0.0], np.float64)
+        self.struct = _FilterPrograms(len(begin) - 1, _p(self.begin), _p(self.nodes), len(values), _p(self.off), _p(self.bytes), _p(self.num))
+
+
+def encode_filters(index, filters, denied=()):
+    """b200_filter_programs of filters (strings for parse_filter, trees, or None for no filter), lowered as a Rust shim lowers
+    FilterCondition: a field absent from the index's fields map is an EMPTY leaf; `denied` holds (field, feature) pairs whose
+    FilterableAttributesFeatures forbid the feature (comparison, equality, exists, null, empty), which become DENIED leaves;
+    CONTAINS, STARTS WITH, _geoPolygon, the resolution argument, _vectors and _shard become UNSUPPORTED leaves"""
+    from .filter import parse_filter
+
+    denied = set(denied)
+    nodes, begin, values = [], [0], []
+
+    def node(op, **kw):
+        x = np.zeros((), FILTER_NODE)
+        x["op"] = op
+        for k, v in kw.items():
+            x[k] = v
+        nodes.append(x)
+        return x
+
+    def emit(t):
+        kind = t[0]
+        if kind in ("and", "or"):
+            node(F_AND if kind == "and" else F_OR, n=len(t[1]))
+            for c in t[1]:
+                emit(c)
+        elif kind == "not":
+            node(F_NOT)
+            emit(t[1])
+        elif kind == "geo":
+            if t[1] in ("radius", "bbox"):
+                args = [float(x) for x in t[2]] + ([0.0] if t[1] == "radius" else [])
+                node(F_GEO_RADIUS if t[1] == "radius" else F_GEO_BBOX, args=args)
+            else:
+                node(F_UNSUPPORTED)
+        else:
+            _, field, op, vals = t
+            if field == "_shard" or field == "_vectors" or field.startswith("_vectors.") or op in ("CONTAINS", "STARTS_WITH"):
+                node(F_UNSUPPORTED)
+            elif field not in index._fields:
+                node(F_EMPTY)
+            elif (field, OP_FEATURE[op]) in denied and not (op == "IN" and not vals):
+                node(F_DENIED, fid=index._fields[field])
+            else:
+                fid = index._fields[field]
+                at = len(values)
+                if op in _RANGE:
+                    from .filter import parse_finite_float
+
+                    lo, hi = _RANGE[op]
+                    pair = vals if op == "TO" else vals * 2
+                    has = all(parse_finite_float(v) is not None for v in (vals if op == "TO" else vals[:1]))
+                    values.extend(pair)
+                    node(F_RANGE, fid=fid, lo=lo, hi=hi, has_number=int(has), value=at)
+                elif op in ("=", "!=", "IN"):
+                    values.extend(vals)
+                    node({"=": F_EQUAL, "!=": F_NOT_EQUAL, "IN": F_IN}[op], fid=fid, value=at, n=len(vals))
+                else:
+                    node({"EXISTS": F_EXISTS, "NULL": F_IS_NULL, "EMPTY": F_IS_EMPTY}[op], fid=fid)
+
+    for f in filters:
+        if f is not None:
+            emit(parse_filter(f) if isinstance(f, str) else f)
+        begin.append(len(nodes))
+    return _Programs(nodes, begin, values)
 
 
 FACET_ORDERS = {"alpha": 0, "count": 1}  # OrderBy::Lexicographic / OrderBy::Count (sortFacetValuesBy)
@@ -264,6 +368,7 @@ class SearchResult:
         self.n_candidates = np.zeros(n, np.uint64)
         self.semantic_hit_count = np.zeros(n, np.uint32)
         self.status = np.zeros(n, np.int32)
+        self.filter_error_leaf = None  # with Search.filter: per query the failing filter leaf, -1 for none
         self.degraded = np.zeros(n, np.uint8)
         self.used_negative_operator = np.zeros(n, np.uint8)
         self.candidates = None  # (n, words) uint64 when requested with Search.with_candidates()
@@ -350,7 +455,9 @@ class Index:
             for is_string, (dbid, db) in enumerate(((DB_FACET_F64, facets.f64_db), (DB_FACET_STRING, facets.string_db))):
                 self._ck(l.b200_stage_db(self._h, dbid, db.n_keys, _p(db.key_bytes), _p(db.key_offsets), _p(db.val_bytes), _p(db.val_offsets)))
                 self._level0[is_string] = [db.key(i) for i in range(db.n_keys) if db.key(i)[2] == 0]
-            for dbid, db in ((DB_FACET_NORMALIZED, getattr(facets, "norm_db", None)), (DB_FACET_ORIGINALS, getattr(facets, "orig_db", None))):
+            for dbid, db in ((DB_FACET_NORMALIZED, getattr(facets, "norm_db", None)), (DB_FACET_ORIGINALS, getattr(facets, "orig_db", None)),
+                             (DB_FACET_EXISTS, getattr(facets, "exists_db", None)), (DB_FACET_IS_NULL, getattr(facets, "null_db", None)),
+                             (DB_FACET_IS_EMPTY, getattr(facets, "empty_db", None))):
                 if db is not None:
                     self._ck(l.b200_stage_db(self._h, dbid, db.n_keys, _p(db.key_bytes), _p(db.key_offsets), _p(db.val_bytes), _p(db.val_offsets)))
         self._n_docs = int(image.n_docs)
@@ -534,6 +641,18 @@ class Index:
         self._ck(self._l.b200_geo_filter_batch(self._h, n, _p(kind), _p(args), _p(out), words, _p(status)))
         return out, status[:n]
 
+    def filter_batch(self, filters, denied=()):
+        """IndexFilter::evaluate over documents_ids (b200_filter_batch): one filter per entry (a string for parse_filter, or a tree it
+        returns; None = no filter) -> (uint64 bitmaps [n, words], statuses [n], failing leaves [n]); see encode_filters for `denied`"""
+        prog = encode_filters(self, list(filters), denied)
+        n = len(filters)
+        words = (self._n_docs + 63) // 64
+        out = np.zeros((n, words), np.uint64)
+        status = np.zeros(max(n, 1), np.int32)
+        leaf = np.zeros(max(n, 1), np.int32)
+        self._ck(self._l.b200_filter_batch(self._h, C.byref(prog.struct), _p(out), words, _p(status), _p(leaf)))
+        return out, status[:n], leaf[:n]
+
     def last_error(self):
         return self._l.b200_last_error(self._h).decode()
 
@@ -695,6 +814,7 @@ class Search:
         self._sort = None
         self._geo_strategy, self._geo_max_bucket = (0, 1000), 1000
         self._geo_filter = None
+        self._filter = None
         self._facet_names, self._max_values, self._facet_order, self._facet_cap = None, DEFAULT_VALUES_PER_FACET, "alpha", None
         self._fsearch = None
 
@@ -760,6 +880,12 @@ class Search:
         """geo leaves at the top of the filter, ANDed with the universe: ["_geoRadius(48.85, 2.35, 2000)", "NOT _geoBoundingBox([1, 2],
         [0, 1])"] for every query of the batch, or one such list per query (see parse_geo_filter)"""
         self._geo_filter = clauses
+        return self
+
+    def filter(self, trees, denied=()):
+        """the `filter` search parameter: one filter (a string for parse_filter, or a tree it returns) for every query of the batch,
+        or a list with one per query (None: no filter); see encode_filters for `denied`"""
+        self._filter = (trees, denied)
         return self
 
     def facet_search(self, name, query=None, order="alpha", max_values=DEFAULT_MAX_FACET_SEARCH_VALUES, typos=True):
@@ -853,6 +979,13 @@ class Search:
             args = np.asarray([a for _, _, a in flat] or [(0.0,) * 4], np.float64).reshape(-1)
             keep += [begin, kind, neg, args]
             b.geo_filter_begin, b.geo_filter_kind, b.geo_filter_not, b.geo_filter_args = _p(begin), _p(kind), _p(neg), _p(args)
+        if self._filter is not None:
+            trees, denied = self._filter
+            per_q = list(trees) if isinstance(trees, list) else [trees] * n
+            prog = encode_filters(ix, per_q, denied)
+            keep.append(prog)
+            b.filter = C.cast(C.pointer(prog.struct), C.c_void_p)
+            res.filter_error_leaf = np.full(max(n, 1), -1, np.int32)
         b.geo_strategy, b.geo_cache_size = self._geo_strategy
         b.geo_max_bucket_size = self._geo_max_bucket
         b.time_budget_ns = 0 if self._budget_ms is None else max(1, int(self._budget_ms * 1e6))
@@ -890,6 +1023,8 @@ class Search:
             b.facet_search_flags, b.facet_search_max = _p(flags), mx
             r.fs_n, r.fs_key, r.fs_count, r.fs_docid, r.fs_fallback = (_p(a) for a in outs)
             res._facet_search = (ix, [(int(fid[q]), qs[q]) for q in range(n)], outs + (mx,))
+        if self._filter is not None:
+            r.filter_error_leaf = _p(res.filter_error_leaf)
         if self._want_candidates:
             words = (ix._n_docs + 63) // 64
             res.candidates = np.zeros((n, words), np.uint64)

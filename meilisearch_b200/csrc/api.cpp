@@ -96,6 +96,7 @@ int b200_stage_db(b200_index *h, int db, uint64_t n, const uint8_t *kb, const ui
         for (uint64_t i = 0; i < n; i++)
             if (ko[i + 1] < ko[i] || vo[i + 1] < vo[i]) return h->e.fail(B200_ERR_INVALID, "stage_db: offsets must not decrease");
         RawDb &d = h->e.raw_dbs[db];
+        d.staged = true;
         d.n = n;
         d.koff.assign(ko, ko + n + 1);
         d.voff.assign(vo, vo + n + 1);
@@ -276,6 +277,7 @@ int b200_search_batch(b200_index *h, const b200_query_batch *b, b200_results *r)
         for (uint32_t i = 0; i < b->n_queries; i++) {
             r->n_hits[i] = 0;
             if (r->status) r->status[i] = 0;
+            if (r->filter_error_leaf) r->filter_error_leaf[i] = -1;
         }
         return h->e.search_batch(b, r);
     });
@@ -285,6 +287,13 @@ int b200_geo_filter_batch(b200_index *h, uint32_t n, const uint8_t *kind, const 
         std::lock_guard<std::mutex> g(h->e.mu);
         if (!h->e.staged) return h->e.fail(B200_ERR_STATE, "geo filter before b200_stage_finish");
         return h->e.geo_filter_batch(n, kind, args, out, out_words, status);
+    });
+}
+int b200_filter_batch(b200_index *h, const b200_filter_programs *programs, uint64_t *out, uint64_t out_words, int32_t *status, int32_t *error_leaf) {
+    return guarded(h, [&]() -> int {
+        std::lock_guard<std::mutex> g(h->e.mu);
+        if (!h->e.staged) return h->e.fail(B200_ERR_STATE, "filter before b200_stage_finish");
+        return h->e.filter_batch(programs, out, out_words, status, error_leaf);
     });
 }
 int b200_facet_distribution_batch(b200_index *h, uint32_t n, const uint64_t *const *candidates, uint64_t n_words, const uint32_t *facet_begin,
@@ -511,19 +520,24 @@ int compare_scores(const Hit &l, float lr, const Hit &r, float rr) {  // hybrid.
 
 // Search::execute_hybrid (search/hybrid.rs:264-366)
 int Engine::search_batch(const b200_query_batch *b, b200_results *r) {
-    if (!b->geo_filter_begin) return search_batch_filtered(b, r);
-    // geo filters: every query's filtered universe is computed once, before the modes split (hybrid runs both stages on it)
+    if (!b->geo_filter_begin && !b->filter) return search_batch_filtered(b, r);
+    // geo filters and filter programs: every query's filtered universe is computed once, before the modes split (hybrid runs both
+    // stages on it)
     cudaError_t e = cudaSetDevice(device);
     if (e != cudaSuccess) return cuda_fail(e, "cudaSetDevice");
     GeoFiltered gf;
-    int rc = geo_filter_universes(b, gf);
+    int rc = b->geo_filter_begin ? geo_filter_universes(b, gf) : B200_OK;
+    if (rc == B200_OK && b->filter) rc = filter_universes(b, gf);
     if (rc != B200_OK) return rc;
     struct Scope {
         const GeoFiltered *&p;
         ~Scope() { p = nullptr; }
     } scope{geo_filtered};
     geo_filtered = &gf;
-    return search_batch_filtered(b, r);
+    rc = search_batch_filtered(b, r);
+    if (r->filter_error_leaf && !gf.error_leaf.empty())
+        for (uint32_t q = 0; q < b->n_queries; q++) r->filter_error_leaf[q] = gf.status[q] ? gf.error_leaf[q] : -1;
+    return rc;
 }
 
 int Engine::search_batch_filtered(const b200_query_batch *b, b200_results *r) {

@@ -241,6 +241,37 @@ struct GeoSlot {
     uint32_t c_begin, c_end;
 };
 
+// ---- filter programs (filter.cu): the tree of a filter as a straight-line program over one-bit registers per document
+constexpr uint16_t FILTER_NO_REG = 0xffff;  // hint register of a node evaluated without a universe hint
+constexpr uint32_t FILTER_REG_WORDS = 63;   // 2016 registers: a program of depth B200_MAX_FILTER_DEPTH needs depth + 1
+enum : uint16_t {
+    FOP_ZERO = 0,    // dst = 0
+    FOP_VALUE = 1,   // dst = the document has an ordinal in intervals [a, b) of iv (doc_off / doc_ord: the field's CSR; nullptr: none);
+                     // neg: docs AND NOT that; hint != FILTER_NO_REG: AND hint
+    FOP_BITMAP = 2,  // dst = bit of bm (nullptr: 0); hint != FILTER_NO_REG: AND hint
+    FOP_AND = 3,     // dst &= src
+    FOP_OR = 4,      // dst |= src
+    FOP_NOT = 5,     // dst = (hint, or docs when FILTER_NO_REG) AND NOT dst
+    FOP_FLAG = 6,    // flag a of the slot = 1 when dst is set for any document
+};
+struct FilterOp {
+    uint16_t code, dst, src, hint;
+    uint32_t a, b;
+    uint32_t neg, pad;
+    const uint32_t *doc_off, *doc_ord;
+    const unsigned long long *bm;
+};
+// one filtered universe: ub AND the program ops[op_begin, op_end) (result in register 0), written to dst, its popcount added to
+// *count; the program's flags live at flags[0 ..); all: every document is evaluated (the flags need the whole document range)
+struct FilterSlot {
+    const unsigned long long *ub;
+    unsigned long long *dst;
+    unsigned long long *count;
+    uint32_t *flags;
+    uint32_t op_begin, op_end;
+    uint32_t all, pad;
+};
+
 // ---- facet distribution (facet.cu): one slot = one (candidate bitmap, faceted field)
 constexpr uint32_t FACET_CANDIDATES_THRESHOLD = 3000;  // facet_distribution.rs:32 CANDIDATES_THRESHOLD
 constexpr uint32_t FACET_SHARED_VALUES = 2048;         // fields with at most this many values count in shared memory

@@ -342,6 +342,9 @@ struct NcclId {
     char internal[128];
 };
 
+// geo filter clause validation (engine_geo.cpp): 0, or B200_ERR_INVALID with the reference's message
+int geo_clause(uint8_t kind, uint8_t neg, const double *a, GeoClause &c, std::string &err);
+
 struct GraphObj;  // S1: opaque query graph (engine_search.cpp)
 void free_graph(GraphObj *);
 
@@ -522,6 +525,7 @@ struct Engine {
         std::vector<uint64_t> count;                     // its cardinality
         std::vector<int32_t> status;                     // B200_ERR_INVALID: a bad clause, or geo not filterable
         std::vector<std::string> error;
+        std::vector<int32_t> error_leaf;                 // filter programs: the leaf whose error failed the query, -1 (may be empty)
     };
     const GeoFiltered *geo_filtered = nullptr;
     bool geo_filterable() const;  // b200_stage_geo_fields named both fields
@@ -530,6 +534,22 @@ struct Engine {
                        std::vector<uint64_t> &counts);
     int geo_filter_universes(const b200_query_batch *b, GeoFiltered &out);
     int geo_filter_batch(uint32_t n, const uint8_t *kind, const double *args, uint64_t *out, uint64_t out_words, int32_t *status);
+    int geo_clause_bitmaps(uint32_t n, const uint8_t *kind, const double *args, DevBuf<unsigned long long> &buf, std::vector<uint32_t> &slot_of,
+                           int32_t *status, std::vector<std::string> &err);
+    // filter programs (filter.cu, engine_filter.cpp): per field its EXISTS / IS NULL / IS EMPTY bitmap; per call the programs' ops,
+    // intervals, slots, flags and counts, the callers' universes AND documents_ids, the slots' bitmaps and the geo leaves' bitmaps
+    std::map<uint16_t, unsigned long long *> d_presence[3];
+    DevBuf<FilterOp> d_ft_op;
+    DevBuf<uint2> d_ft_iv;
+    DevBuf<FilterSlot> d_ft_slot;
+    DevBuf<uint32_t> d_ft_flag;
+    DevBuf<unsigned long long> d_ft_count, d_ft_caller, d_ft_univ, d_ft_geo;
+    // program q of `p` over base[q] (a device bitmap; nullptr: no program for q) into gf (d_univ, count, status, error, error_leaf);
+    // queries whose gf.status is already set are skipped
+    int run_filters(const b200_filter_programs *p, const std::vector<const unsigned long long *> &base, GeoFiltered &gf);
+    // search_batch: every query's universe with its program applied (after geo_filter_universes when the batch has geo clauses)
+    int filter_universes(const b200_query_batch *b, GeoFiltered &gf);
+    int filter_batch(const b200_filter_programs *p, uint64_t *out, uint64_t out_words, int32_t *status, int32_t *error_leaf);
     // facet distribution (facet.cu, engine_facet.cpp).  A slot is one (candidate bitmap on the device, field); its outputs sit at
     // index `slot` of the device outputs, which facet_results copies back and decodes into the caller's b200_results::facet_* arrays.
     struct FacetJob {

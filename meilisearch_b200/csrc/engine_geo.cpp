@@ -53,6 +53,8 @@ void geo_radius_band(double r_eps, double &lo, double &hi) {
     hi = b < M_PI - 1e-4 ? std::pow(2.0 * std::sin(b / 2.0), 2) * (1.0 + 1e-12) : HUGE_VAL;
 }
 
+}  // namespace
+
 // One clause from the ABI's (kind, four doubles), validated in the reference's order: the coordinates finite, then their ranges, then
 // the radius (finite) or top >= bottom.  Returns 0 or B200_ERR_INVALID with the reference's message.
 int geo_clause(uint8_t kind, uint8_t neg, const double *a, GeoClause &c, std::string &err) {
@@ -105,6 +107,8 @@ int geo_clause(uint8_t kind, uint8_t neg, const double *a, GeoClause &c, std::st
     }
     return B200_OK;
 }
+
+namespace {
 
 // identical clauses share one entry (and one pass-1 search): the key is the clause's defining bytes
 struct ClauseSet {
@@ -247,47 +251,55 @@ int Engine::geo_filter_universes(const b200_query_batch *b, GeoFiltered &gf) {
     return B200_OK;
 }
 
-int Engine::geo_filter_batch(uint32_t n, const uint8_t *kind, const double *args, uint64_t *out, uint64_t out_words, int32_t *status) {
+// One bitmap over documents_ids per valid clause i (kind[i], args[4 i ..)) into buf; slot_of[i] = its bitmap (identical clauses share
+// one), UINT32_MAX for a clause refused with status[i] / err[i].  One synchronise.
+int Engine::geo_clause_bitmaps(uint32_t n, const uint8_t *kind, const double *args, DevBuf<unsigned long long> &buf, std::vector<uint32_t> &slot_of,
+                               int32_t *status, std::vector<std::string> &err) {
     const uint64_t W = hix.n_words64;
-    if (n && (!kind || !args || !out || !status)) return fail(B200_ERR_INVALID, "geo_filter_batch: null kind / args / out / status");
-    if (out_words < W) return fail(B200_ERR_INVALID, "geo_filter_batch: out_words smaller than the document range");
-    CU(cudaSetDevice(device), "cudaSetDevice");
     ClauseSet cs;
-    std::vector<uint32_t> slot_of(n, UINT32_MAX);
+    slot_of.assign(n, UINT32_MAX);
+    err.assign(n, std::string());
     for (uint32_t i = 0; i < n; i++) {
-        memset(out + (size_t)i * out_words, 0, out_words * 8);
         GeoClause c;
-        std::string err;
-        status[i] = geo_clause(kind[i], 0, args + 4 * (size_t)i, c, err);
+        status[i] = geo_clause(kind[i], 0, args + 4 * (size_t)i, c, err[i]);
         if (!status[i] && !geo_filterable()) {
             status[i] = B200_ERR_INVALID;
-            err = NOT_FILTERABLE;
+            err[i] = NOT_FILTERABLE;
         }
-        if (status[i]) {
-            last_error = err;
-            continue;
-        }
-        slot_of[i] = cs.add(kind[i], 0, args + 4 * (size_t)i, c);
+        if (!status[i]) slot_of[i] = cs.add(kind[i], 0, args + 4 * (size_t)i, c);
     }
     if (cs.clauses.empty()) return B200_OK;
-    // one slot per distinct clause, over documents_ids
     const uint32_t n_slots = (uint32_t)cs.clauses.size();
-    int rc = reserve_geo_bitmaps(d_gf_univ, n_slots);
+    int rc = reserve_geo_bitmaps(buf, n_slots);
     if (rc != B200_OK) return rc;
     std::vector<uint32_t> slot_clauses(n_slots);
     std::vector<GeoSlot> slots(n_slots);
     for (uint32_t s = 0; s < n_slots; s++) {
         slot_clauses[s] = s;
-        slots[s] = GeoSlot{dix.base_ub, d_gf_univ.p + (size_t)s * W, nullptr, s, s + 1};
+        slots[s] = GeoSlot{dix.base_ub, buf.p + (size_t)s * W, nullptr, s, s + 1};
     }
     std::vector<uint64_t> counts;
-    rc = run_geo_filter(cs.clauses, slot_clauses, slots, counts);
+    return run_geo_filter(cs.clauses, slot_clauses, slots, counts);
+}
+
+int Engine::geo_filter_batch(uint32_t n, const uint8_t *kind, const double *args, uint64_t *out, uint64_t out_words, int32_t *status) {
+    const uint64_t W = hix.n_words64;
+    if (n && (!kind || !args || !out || !status)) return fail(B200_ERR_INVALID, "geo_filter_batch: null kind / args / out / status");
+    if (out_words < W) return fail(B200_ERR_INVALID, "geo_filter_batch: out_words smaller than the document range");
+    CU(cudaSetDevice(device), "cudaSetDevice");
+    for (uint32_t i = 0; i < n; i++) memset(out + (size_t)i * out_words, 0, out_words * 8);
+    std::vector<uint32_t> slot_of;
+    std::vector<std::string> err;
+    int rc = geo_clause_bitmaps(n, kind, args, d_gf_univ, slot_of, status, err);
     if (rc != B200_OK) return rc;
-    for (uint32_t i = 0; i < n; i++)
-        if (slot_of[i] != UINT32_MAX) {
-            CU(cudaMemcpyAsync(out + (size_t)i * out_words, slots[slot_of[i]].dst, W * 8, cudaMemcpyDeviceToHost, stream), "D2H geo filter");
-            stats.d2h_bytes += W * 8;
+    for (uint32_t i = 0; i < n; i++) {
+        if (status[i]) {
+            last_error = err[i];
+            continue;
         }
+        CU(cudaMemcpyAsync(out + (size_t)i * out_words, d_gf_univ.p + (size_t)slot_of[i] * W, W * 8, cudaMemcpyDeviceToHost, stream), "D2H geo filter");
+        stats.d2h_bytes += W * 8;
+    }
     CU(cudaStreamSynchronize(stream), "sync");
     return B200_OK;
 }

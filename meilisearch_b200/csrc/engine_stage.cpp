@@ -115,6 +115,16 @@ Engine::~Engine() {
     d_gf_count.release();
     d_gf_caller.release();
     d_gf_univ.release();
+    for (auto &m : d_presence)
+        for (auto &kv : m) cudaFree(kv.second);
+    d_ft_op.release();
+    d_ft_iv.release();
+    d_ft_slot.release();
+    d_ft_flag.release();
+    d_ft_count.release();
+    d_ft_caller.release();
+    d_ft_univ.release();
+    d_ft_geo.release();
     for (auto &ln : lanes) ln.release();
     d_docids_out.release();
     d_sort_desc.release();
@@ -189,6 +199,7 @@ int Engine::stage_finish() {
         build_geo_field(raw_dbs[B200_DB_FACET_ID_F64_DOCIDS], raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], hix);
         build_facet_search(raw_dbs[B200_DB_FACET_ID_STRING_DOCIDS], raw_dbs[B200_DB_FACET_ID_NORMALIZED_STRING_STRINGS],
                            raw_dbs[B200_DB_FIELD_ID_DOCID_FACET_STRINGS], hix);
+        for (int p = 0; p < 3; p++) build_presence(raw_dbs[B200_DB_FACET_ID_EXISTS_DOCIDS + p], p, hix);
     } catch (const std::exception &e) {
         return fail(B200_ERR_INVALID, e.what());
     }
@@ -225,10 +236,19 @@ int Engine::stage_finish() {
         CU(upload(&f.d_doc_ord, src(f.doc_ord), f.doc_ord.size()), "upload facet ordinals");
         CU(upload(&f.d_disp, src(f.disp), f.disp.size()), "upload facet display order");
         stats.hbm_bytes_staged += (f.doc_off.size() + f.doc_ord.size() + f.disp.size()) * 4;
+        f.n_ord = f.doc_ord.size();
         std::vector<uint32_t>().swap(f.doc_off);
         std::vector<uint32_t>().swap(f.doc_ord);
         std::vector<uint32_t>().swap(f.disp);
     }
+    // filters: the EXISTS / IS NULL / IS EMPTY bitmaps of every field
+    for (int p = 0; p < 3; p++)
+        for (auto &kv : hix.presence[p]) {
+            CU(upload(&d_presence[p][kv.first], reinterpret_cast<const unsigned long long *>(kv.second.data()), kv.second.size()),
+               "upload facet presence");
+            stats.hbm_bytes_staged += kv.second.size() * 8;
+            std::vector<uint64_t>().swap(kv.second);
+        }
     // facet search: the hyper-normalised strings as chars and the keys each one walks (the keys' posting lists are in the pool,
     // counted above)
     {

@@ -318,12 +318,27 @@ void build_host_index(const std::vector<uint8_t> &dict_bytes, const std::vector<
     }
 }
 
+void build_presence(const RawDb &db, int which, HostIndex &ix) {
+    std::vector<uint32_t> docs;
+    for (uint64_t i = 0; i < db.n; i++) {
+        const uint8_t *k = db.keys.data() + db.koff[i];
+        if (db.koff[i + 1] - db.koff[i] != 2) throw std::runtime_error("stage: facet presence key is not a u16 BE field id");
+        std::vector<uint64_t> &bm = ix.presence[which][(uint16_t)(k[0] << 8 | k[1])];
+        bm.assign(ix.n_words64, 0);
+        docs.clear();
+        cbo_decode_append(db.vals.data() + db.voff[i], db.voff[i + 1] - db.voff[i], docs);
+        for (uint32_t d : docs)
+            if (d < ix.n_docs) bm[d >> 6] |= 1ull << (d & 63);
+    }
+}
+
 void build_sort_fields(const RawDb &f64_db, const RawDb &string_db, HostIndex &ix) {
     ix.sort_fields.clear();
     struct Val {
         uint16_t fid;
         uint32_t key_index;  // among the level-0 keys of its database
         std::vector<uint32_t> docs;
+        std::string bound;  // strings: the normalised key
     };
     // level-0 entries in LMDB order (u16 BE fid | u8 level | bound): per field, numbers and strings each come in ascending order
     auto level0 = [&](const RawDb &db, bool numbers) {
@@ -341,6 +356,7 @@ void build_sort_fields(const RawDb &f64_db, const RawDb &string_db, HostIndex &i
             Val x;
             x.fid = (uint16_t)(k[0] << 8 | k[1]);
             x.key_index = l0++;
+            if (!numbers) x.bound.assign((const char *)k + 3, kn - 3);
             cbo_decode_append(v + 1, vn - 1, x.docs);
             out.push_back(std::move(x));
         }
@@ -355,6 +371,7 @@ void build_sort_fields(const RawDb &f64_db, const RawDb &string_db, HostIndex &i
     for (auto &x : strs) {
         SortField &f = ix.sort_fields[x.fid];
         f.str_key.push_back(x.key_index);
+        f.str_val.push_back(x.bound);
         f.n_str++;
     }
     for (auto &kv : ix.sort_fields) {

@@ -26,6 +26,7 @@ struct ListRef {
 };
 
 struct RawDb {
+    bool staged = false;  // b200_stage_db was called for it
     uint64_t n = 0;
     std::vector<uint8_t> keys, vals;
     std::vector<uint64_t> koff, voff;
@@ -64,6 +65,8 @@ struct SortField {
     std::vector<uint32_t> doc_off, doc_ord, disp;
     uint32_t *d_doc_off = nullptr, *d_doc_ord = nullptr, *d_disp = nullptr;
     std::vector<double> num_val;
+    std::vector<std::string> str_val;  // the string ordinals' normalised keys (filters bound them in byte order)
+    uint64_t n_ord = 0;                // doc_ord's length (kept after upload)
     uint32_t n_values() const { return n_num + n_str; }
     // ordinal of direction `asc` -> (is_string, position among the level-0 keys of its database)
     void decode(bool asc, uint32_t o, bool &is_string, uint32_t &key_index) const {
@@ -138,6 +141,8 @@ struct HostIndex {
     std::map<uint16_t, SortField> sort_fields;  // faceted fields (fid -> SortField)
     GeoField geo;
     FacetSearchIndex fsearch;
+    // facet_id_{exists,is_null,is_empty}_docids: fid -> dense bitmap of n_words64 words (released after upload)
+    std::map<uint16_t, std::vector<uint64_t>> presence[3];
     // list id of key i of database db = db_first[db] + i (keys in LMDB order); db_keys[db] = number of staged keys.
     // (word_pair_proximity keys naming unknown words are dropped at staging: for that db the mapping only holds when none was.)
     uint32_t db_first[10] = {0}, db_keys[10] = {0};
@@ -237,6 +242,9 @@ void build_host_index(const std::vector<uint8_t> &dict_bytes, const std::vector<
 // Decode the level-0 entries of facet_id_f64_docids / facet_id_string_docids into out.sort_fields (after build_host_index: needs
 // n_docs).  Throws std::runtime_error on a malformed key or value.
 void build_sort_fields(const RawDb &f64_db, const RawDb &string_db, HostIndex &out);
+// Decode facet_id_exists_docids / facet_id_is_null_docids / facet_id_is_empty_docids (key u16 BE fid, value CBO) into
+// out.presence[which] (after build_host_index: needs n_words64).  Throws std::runtime_error on a malformed key.
+void build_presence(const RawDb &db, int which, HostIndex &out);
 // Rust's `impl Display for f64`: the shortest digits that read back as the same value, never an exponent ("-0" for -0.0)
 std::string rust_f64_display(double v);
 // Read every document's point into out.geo (after build_host_index; out.geo.lat_fid / lng_fid set, or nothing to do).  Throws

@@ -39,6 +39,9 @@ cudaError_t launch_geo_first_fail(cudaStream_t s, const unsigned long long *geo,
                                   const uint32_t *radius, uint32_t n_radius, GeoFirst *first);
 cudaError_t launch_geo_filter(cudaStream_t s, const unsigned long long *geo, const GeoPoint *pts, uint32_t n_words, const GeoClause *clauses,
                               const GeoFirst *first, const uint32_t *slot_clauses, const GeoSlot *slots, uint32_t n_slots);
+// filter.cu: every slot's filtered universe (FilterSlot: counts and flags zero at launch); docs = documents_ids
+cudaError_t launch_filter(cudaStream_t s, const FilterOp *ops, const uint2 *iv, const FilterSlot *slots, uint32_t n_slots,
+                          const unsigned long long *docs, uint32_t n_docs, uint32_t n_words);
 // facet.cu: counts of every slot's values over its candidates (FacetSlot scratch zero at launch), then one CTA per slot selects the
 // entries the reference's facet_values returns
 cudaError_t launch_facet(cudaStream_t s, const FacetSlot *slots, uint32_t n_slots, uint32_t n_words, uint32_t n_docs);
