@@ -457,6 +457,40 @@ int b200_facet_search_batch(b200_index *, uint32_t n, const uint64_t *const *can
                             uint32_t cap, uint32_t *n_out, uint32_t *key, uint64_t *count, uint32_t *docid, uint8_t *fallback,
                             int32_t *status);
 
+/* Replaces Similar::execute (crates/milli/src/search/similar.rs:66-152), as called by perform_similar
+ * (crates/meilisearch/src/search/mod.rs:2577-2735), with VectorStore::nns_by_item (vector/store.rs:615-637,980-1034) answered by an
+ * exact scan of the staged store.  For query i, target `id` = docids[i] and U = documents_ids AND universes[i] AND program i of
+ * `filter` (b200_query_batch semantics for both; filter->n == n_queries):
+ *   1. the universe is U \ {id};
+ *   2. the query is the target's staged row; the candidate list is the nearest offset + limit + 1 rows of U \ {id}, ascending by
+ *      (distance, docid), distance (1 - cos) / 2 with the norm rule of b200_nns_batch;
+ *   3. the list is walked in order: `seen` starts as {id}, a docid already in it is dropped, otherwise added (before the skip and the
+ *      take); the first `offset` survivors are skipped (still added to `seen`); at most `limit` are taken, each with score
+ *      1 - distance, shifted by the staged distribution if there is one.  With a threshold, a taken document whose score is below it
+ *      ends the walk and sets candidates = (candidates \ {doc}) AND seen; skipped documents are never tested;
+ *   4. outputs: the hits in b200_results::docids (stride `limit`) and n_hits, one B200_S_VECTOR score per hit (n_scores = 1,
+ *      score_sim = the score, which is also the global score), n_candidates = |candidates|, candidates starting as U \ {id} (the
+ *      route's estimatedTotalHits).  Unembedded documents are never returned (unlike VectorSort's last bucket in searches);
+ *   5. a target without an embedding, outside documents_ids or beyond the document range has no hits, n_candidates = |U \ {id}| and
+ *      status 0, as nns_by_item answers for an absent item.
+ * The reference scans once per store, store k holding each document's k-th vector and searched with the target's k-th vector; the
+ * staged store is flat, so on a store where a document has more than one row every query fails alone with B200_ERR_UNSUPPORTED.
+ * Per query, as in searches: filter errors (filter_error_leaf names the node).  For the call: B200_ERR_INVALID for NULL docids or
+ * universes shorter than the document range, B200_ERR_STATE before b200_stage_finish or without staged embeddings,
+ * B200_ERR_UNSUPPORTED for a non-NULL b200_results::candidates (the route reads only its length).  The target's vector never crosses
+ * PCIe: the scan gathers it from HBM. */
+typedef struct {
+    uint32_t n_queries;
+    const uint32_t *docids;          /* n_queries internal docids of the target documents */
+    uint32_t offset, limit;
+    const uint64_t *const *universes; /* as b200_query_batch::universes (NULL array / entry: documents_ids) */
+    uint64_t n_universe_words;
+    const b200_filter_programs *filter; /* as b200_query_batch::filter (NULL = none) */
+    int32_t has_ranking_score_threshold;
+    double ranking_score_threshold;
+} b200_similar_request;
+int b200_similar_batch(b200_index *, const b200_similar_request *, b200_results *);
+
 /* ---- S1: the RankingRule seam ---------------------------------------------------------- */
 /* Replaces `dyn RankingRule` as driven by bucket_sort (crates/milli/src/search/new/ranking_rules.rs:26-83, bucket_sort.rs:123,266,323)
  * for the graph-based rules and ExactAttribute.  Query graphs are opaque library objects (a QueryGraph plus the terms it refers

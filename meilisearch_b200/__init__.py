@@ -73,6 +73,12 @@ class _FilterPrograms(C.Structure):
                 ("value_bytes", C.c_void_p), ("value_num", C.c_void_p)]
 
 
+class _SimilarRequest(C.Structure):
+    _fields_ = [("n_queries", C.c_uint32), ("docids", C.c_void_p), ("offset", C.c_uint32), ("limit", C.c_uint32), ("universes", C.c_void_p),
+                ("n_universe_words", C.c_uint64), ("filter", C.c_void_p), ("has_ranking_score_threshold", C.c_int32),
+                ("ranking_score_threshold", C.c_double)]
+
+
 class _Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("device_steps", C.c_uint64), ("posting_bytes", C.c_uint64), ("matrix_bytes", C.c_uint64),
                 ("dictionary_bytes", C.c_uint64), ("vector_bytes", C.c_uint64), ("kernel_ms", C.c_double * 16),
@@ -132,6 +138,7 @@ def load_library():
                                                     C.c_uint32] + [C.c_void_p] * 9
         l.b200_facet_search_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64] + [C.c_void_p] * 5 + [C.c_uint32, C.c_uint32] + \
             [C.c_void_p] * 6
+        l.b200_similar_batch.argtypes = [C.c_void_p, C.POINTER(_SimilarRequest), C.POINTER(_Results)]
         l.b200_proximity_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
         l.b200_graph_from_tokens.argtypes = [C.c_void_p, C.POINTER(_Batch), C.POINTER(C.c_void_p)]
         l.b200_graph_free.argtypes = [C.c_void_p]
@@ -146,7 +153,7 @@ def load_library():
 
 SYMBOLS = ["b200_open", "b200_close", "b200_last_error", "b200_open_error", "b200_stage_dictionary", "b200_stage_db",
            "b200_stage_documents_ids", "b200_stage_settings", "b200_stage_synonyms", "b200_stage_geo_fields", "b200_stage_finish", "b200_stage_embeddings", "b200_stage_embeddings_f16", "b200_stage_distribution",
-           "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_geo_filter_batch", "b200_filter_batch", "b200_facet_distribution_batch", "b200_facet_search_batch", "b200_graph_from_tokens",
+           "b200_derive_batch", "b200_union_postings", "b200_proximity_pairs", "b200_nns_batch", "b200_nns_batch_sharded", "b200_comm_unique_id", "b200_comm_init", "b200_search_batch", "b200_geo_filter_batch", "b200_filter_batch", "b200_facet_distribution_batch", "b200_facet_search_batch", "b200_similar_batch", "b200_graph_from_tokens",
            "b200_graph_free", "b200_rule_start", "b200_rule_next", "b200_rule_end", "b200_get_stats", "b200_reset_stats"]
 
 
@@ -622,6 +629,41 @@ class Index:
         cw = None if candidates is None else np.ascontiguousarray(candidates, np.uint64)
         self._ck(self._l.b200_nns_batch_sharded(self._h, _p(q), n, q.shape[1], limit, _p(cw), 0 if cw is None else len(cw), _p(ids), _p(dist), _p(cnt)))
         return ids, dist, cnt
+
+    def similar(self, ids, *, offset=0, limit=20, filter=None, universes=None, ranking_score_threshold=None, denied=()):
+        """Similar::execute (search/similar.rs:66-152) for a batch of target documents (internal docids), as the `/similar` route
+        runs it (b200_similar_batch): the nearest documents to each target's stored vector, the target left out.  filter: one filter
+        (a string for parse_filter, or a tree it returns) for every target, or a list with one per target (None: no filter), see
+        encode_filters for `denied`; universes: as Search.universes.  Returns a SearchResult (one Vector score per hit,
+        n_candidates = estimatedTotalHits)."""
+        targets = np.ascontiguousarray(np.atleast_1d(ids), np.uint32)
+        n = len(targets)
+        res = SearchResult(n, limit)
+        rq = _SimilarRequest(n, _p(targets), offset, limit)
+        keep = []
+        if universes is not None:
+            us = [universes] * n if isinstance(universes, np.ndarray) and universes.ndim == 1 else universes
+            ptrs = (C.c_void_p * max(n, 1))()
+            cache = {}
+            for i, u in enumerate(us):
+                if u is not None:
+                    a = cache.setdefault(id(u), np.ascontiguousarray(u, np.uint64))
+                    ptrs[i] = a.ctypes.data
+                    rq.n_universe_words = len(a)
+            keep += [cache, ptrs]
+            rq.universes = C.cast(ptrs, C.c_void_p)
+        r = _Results(_p(res.documents_ids), _p(res.n_hits), _p(res.n_scores), _p(res.score_kind), _p(res.score_rank), _p(res.score_max),
+                     _p(res.score_sim), _p(res.n_candidates), None, _p(res.status))
+        if filter is not None:
+            prog = encode_filters(self, list(filter) if isinstance(filter, list) else [filter] * n, denied)
+            keep.append(prog)
+            rq.filter = C.cast(C.pointer(prog.struct), C.c_void_p)
+            res.filter_error_leaf = np.full(max(n, 1), -1, np.int32)
+            r.filter_error_leaf = _p(res.filter_error_leaf)
+        rq.has_ranking_score_threshold = int(ranking_score_threshold is not None)
+        rq.ranking_score_threshold = float(ranking_score_threshold or 0.0)
+        self._ck(self._l.b200_similar_batch(self._h, C.byref(rq), C.byref(r)))
+        return res
 
     def search(self):
         return Search(self)

@@ -5,8 +5,10 @@
 #include <cstring>
 #include <map>
 #include <new>
+#include <unordered_set>
 
 #include "engine.h"
+#include "kernels.h"
 
 using namespace b200;
 
@@ -326,6 +328,21 @@ int b200_facet_search_batch(b200_index *h, uint32_t n, const uint64_t *const *ca
                                        fallback, status);
     });
 }
+int b200_similar_batch(b200_index *h, const b200_similar_request *rq, b200_results *r) {
+    return guarded(h, [&]() -> int {
+        std::lock_guard<std::mutex> g(h->e.mu);
+        if (!rq || !r || !r->n_hits || (rq->n_queries && rq->limit && !r->docids)) return h->e.fail(B200_ERR_INVALID, "similar: null request / results / docids / n_hits");
+        if (!h->e.staged) return h->e.fail(B200_ERR_STATE, "similar before b200_stage_finish");
+        for (uint32_t i = 0; i < rq->n_queries; i++) {
+            r->n_hits[i] = 0;
+            if (r->status) r->status[i] = 0;
+            if (r->filter_error_leaf) r->filter_error_leaf[i] = -1;
+        }
+        int rc = h->e.similar_batch(rq, r);
+        h->e.fold_vector_stats();
+        return rc;
+    });
+}
 int b200_get_stats(b200_index *h, b200_stats *out) {
     std::lock_guard<std::mutex> g(h->e.mu);
     *out = h->e.stats;
@@ -351,6 +368,29 @@ static float distribution_shift(float mean, float sigma, float score) {  // vect
     return s;
 }
 
+std::vector<Engine::UniverseGroup> Engine::group_by_universe(uint32_t n_queries, const uint64_t *const *universes, const GeoFiltered *gf) const {
+    std::map<std::pair<const uint64_t *, const unsigned long long *>, std::vector<uint32_t>> groups;
+    for (uint32_t q = 0; q < n_queries; q++) {
+        if (gf && gf->status[q]) continue;
+        if (gf && gf->d_univ[q])
+            groups[{nullptr, gf->d_univ[q]}].push_back(q);
+        else
+            groups[{universes ? universes[q] : nullptr, nullptr}].push_back(q);
+    }
+    std::vector<UniverseGroup> out;
+    for (auto &g : groups) {
+        UniverseGroup u{g.first.first, g.first.second, hix.n_documents, std::move(g.second)};
+        if (u.dev) {
+            u.count = gf->count[u.queries[0]];
+        } else if (u.host) {
+            u.count = 0;
+            for (uint64_t w = 0; w < hix.n_words64; w++) u.count += (uint64_t)__builtin_popcountll(u.host[w] & hix.base_ub[w]);
+        }
+        out.push_back(std::move(u));
+    }
+    return out;
+}
+
 // execute_vector_search (search/new/mod.rs:744-808): one VectorSort rule over documents_ids; buckets = runs of equal
 // distance in ascending docid order (vector_sort.rs:80-95), which the (distance, docid) ordering of nns_batch reproduces.
 int Engine::semantic_batch(const b200_query_batch *b, b200_results *r, uint32_t offset, uint32_t limit) {
@@ -368,36 +408,19 @@ int Engine::semantic_batch(const b200_query_batch *b, b200_results *r, uint32_t 
         // filtered_universe restricts the vector candidates (vector_sort.rs:58-78: `vector_candidates & universe`): the queries
         // are grouped by bitmap (the caller's, or a geo-filtered one on the device) and every group is one scan with that filter
         if (b->universes && b->n_universe_words < hix.n_words64) return fail(B200_ERR_INVALID, "universe bitmaps shorter than the document range");
-        std::map<std::pair<const uint64_t *, const unsigned long long *>, std::vector<uint32_t>> groups;
-        for (uint32_t q = 0; q < b->n_queries; q++) {
-            if (gf && gf->status[q]) continue;
-            if (gf && gf->d_univ[q])
-                groups[{nullptr, gf->d_univ[q]}].push_back(q);
-            else
-                groups[{b->universes ? b->universes[q] : nullptr, nullptr}].push_back(q);
-        }
         const uint32_t d = emb_d_user;
-        for (auto &g : groups) {
-            const uint32_t m = (uint32_t)g.second.size();
+        for (const UniverseGroup &g : group_by_universe(b->n_queries, b->universes, gf)) {
+            const uint32_t m = (uint32_t)g.queries.size();
             std::vector<float> vq((size_t)m * d);
-            for (uint32_t i = 0; i < m; i++) memcpy(vq.data() + (size_t)i * d, b->vectors + (size_t)g.second[i] * d, (size_t)d * 4);
+            for (uint32_t i = 0; i < m; i++) memcpy(vq.data() + (size_t)i * d, b->vectors + (size_t)g.queries[i] * d, (size_t)d * 4);
             std::vector<uint32_t> gi((size_t)m * k), gn(m);
             std::vector<float> gd((size_t)m * k);
-            const uint64_t *hu = g.first.first;
-            const unsigned long long *du = g.first.second;
-            uint64_t cnt = hix.n_documents;
-            if (du) {
-                cnt = gf->count[g.second[0]];
-            } else if (hu) {
-                cnt = 0;
-                for (uint64_t w = 0; w < hix.n_words64; w++) cnt += (uint64_t)__builtin_popcountll(hu[w] & hix.base_ub[w]);
-            }
-            int rc = nns_batch(vq.data(), m, d, k, hu, hu || du ? hix.n_words64 : 0, gi.data(), gd.data(), gn.data(), false, du);
+            int rc = nns_batch(vq.data(), m, d, k, g.host, g.host || g.dev ? hix.n_words64 : 0, gi.data(), gd.data(), gn.data(), false, g.dev);
             if (rc != B200_OK) return rc;
             for (uint32_t i = 0; i < m; i++) {
-                const uint32_t q = g.second[i];
+                const uint32_t q = g.queries[i];
                 n[q] = gn[i];
-                n_cand[q] = cnt;
+                n_cand[q] = g.count;
                 memcpy(ids.data() + (size_t)q * k, gi.data() + (size_t)i * k, (size_t)gn[i] * 4);
                 memcpy(dist.data() + (size_t)q * k, gd.data() + (size_t)i * k, (size_t)gn[i] * 4);
             }
@@ -453,6 +476,138 @@ int Engine::semantic_batch(const b200_query_batch *b, b200_results *r, uint32_t 
                 r->score_max[at * B200_MAX_SCORES] = 1;
                 r->score_sim[at * B200_MAX_SCORES] = sim;
             }
+        }
+    }
+    return B200_OK;
+}
+
+// Similar::execute (search/similar.rs:66-152); semantics in include/b200milli.h (b200_similar_batch)
+int Engine::similar_batch(const b200_similar_request *rq, b200_results *r) {
+    const uint32_t NQ = rq->n_queries;
+    const uint64_t W = hix.n_words64;
+    if (!rq->docids) return fail(B200_ERR_INVALID, "similar: null docids");
+    if (rq->universes && rq->n_universe_words < W) return fail(B200_ERR_INVALID, "universe bitmaps shorter than the document range");
+    if (r->candidates) return fail(B200_ERR_UNSUPPORTED, "similar: the candidates bitmap is not returned (the route reads only its length)");
+    if (!dix.emb) return fail(B200_ERR_STATE, "similar before b200_stage_embeddings");
+    if (cudaError_t e = cudaSetDevice(device)) return cuda_fail(e, "cudaSetDevice");
+    // filtered_universe: the filter programs run exactly as in searches (filter_universes), so their errors fail their query alone
+    GeoFiltered gf;
+    const GeoFiltered *gfp = nullptr;
+    if (rq->filter) {
+        b200_query_batch qb{};
+        qb.n_queries = NQ;
+        qb.universes = rq->universes;
+        qb.n_universe_words = rq->n_universe_words;
+        qb.filter = rq->filter;
+        int rc = filter_universes(&qb, gf);
+        if (rc != B200_OK) return rc;
+        gfp = &gf;
+        if (r->filter_error_leaf && !gf.error_leaf.empty())
+            for (uint32_t q = 0; q < NQ; q++) r->filter_error_leaf[q] = gf.status[q] ? gf.error_leaf[q] : -1;
+    }
+    for (uint32_t q = 0; q < NQ; q++) {
+        r->n_hits[q] = 0;
+        if (r->n_candidates) r->n_candidates[q] = 0;
+        if (r->degraded) r->degraded[q] = 0;
+        if (r->used_negative_operator) r->used_negative_operator[q] = 0;
+        if (r->semantic_hits) r->semantic_hits[q] = 0;
+        int32_t st = gfp ? gf.status[q] : 0;
+        if (st) last_error = gf.error[q];
+        else if (emb_multi_row) {
+            st = B200_ERR_UNSUPPORTED;
+            last_error = "similar: a document has several embeddings (the reference searches each of its stores with the target's vector of that store)";
+        }
+        if (r->status) r->status[q] = st;
+    }
+    if (emb_multi_row) return B200_OK;
+    const auto in = [](const uint64_t *bm, uint32_t doc) { return ((bm[doc >> 6] >> (doc & 63)) & 1) != 0; };
+    const uint32_t offset = rq->offset, limit = rq->limit, keep = offset + limit + 1, k = keep + 1;
+    for (const UniverseGroup &g : group_by_universe(NQ, rq->universes, gfp)) {
+        // |U \ {id}| needs to know whether the target is in U: on the host for the caller's bitmaps, one batched read of the target
+        // words for a device bitmap
+        const uint32_t m = (uint32_t)g.queries.size();
+        std::vector<uint8_t> member(m, 0);
+        std::vector<uint32_t> probe;  // indices into g.queries whose target word is read from the device
+        for (uint32_t i = 0; i < m; i++) {
+            const uint32_t id = rq->docids[g.queries[i]];
+            if (id >= W * 64 || !in(hix.base_ub.data(), id)) continue;  // outside documents_ids, or beyond the document range
+            if (g.dev)
+                probe.push_back(i);
+            else
+                member[i] = !g.host || in(g.host, id);
+        }
+        if (!probe.empty()) {
+            const uint32_t np = (uint32_t)probe.size();
+            std::vector<unsigned long long> addr(np), words(np);
+            for (uint32_t j = 0; j < np; j++) addr[j] = (unsigned long long)(uintptr_t)(g.dev + (rq->docids[g.queries[probe[j]]] >> 6));
+            cudaError_t e = d_sim_addr.reserve(np);
+            if (e == cudaSuccess) e = d_sim_word.reserve(np);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(d_sim_addr.p, addr.data(), (size_t)np * 8, cudaMemcpyHostToDevice, vt.stream);
+            if (e == cudaSuccess) e = launch_gather_words(vt.stream, d_sim_addr.p, np, d_sim_word.p);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(words.data(), d_sim_word.p, (size_t)np * 8, cudaMemcpyDeviceToHost, vt.stream);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(vt.stream);
+            if (e != cudaSuccess) return cuda_fail(e, "similar: target words");
+            vstats.h2d_bytes += (size_t)np * 8;
+            vstats.d2h_bytes += (size_t)np * 8;
+            vstats.kernel_launches++;
+            for (uint32_t j = 0; j < np; j++) member[probe[j]] = (words[j] >> (rq->docids[g.queries[probe[j]]] & 63)) & 1;
+        }
+        // the scan: every embedded target in documents_ids, over the group's universe with the target still in it
+        std::vector<uint32_t> rows, at;
+        for (uint32_t i = 0; i < m; i++) {
+            const uint32_t q = g.queries[i], id = rq->docids[q];
+            if (r->n_candidates) r->n_candidates[q] = g.count - member[i];
+            if (id < W * 64 && in(hix.base_ub.data(), id) && id < emb_row.size() && emb_row[id] != UINT32_MAX) {
+                rows.push_back(emb_row[id]);
+                at.push_back(i);
+            }
+        }
+        if (rows.empty()) continue;
+        // U is always within documents_ids: a caller's bitmap is intersected with it, and without one documents_ids is the filter
+        std::vector<uint64_t> hu;
+        if (g.host) {
+            hu.resize(W);
+            for (uint64_t w = 0; w < W; w++) hu[w] = g.host[w] & hix.base_ub[w];
+        }
+        const unsigned long long *du = g.dev ? g.dev : (g.host ? nullptr : dix.base_ub);
+        const uint32_t nr = (uint32_t)rows.size();
+        std::vector<uint32_t> gi((size_t)nr * k), gn(nr);
+        std::vector<float> gd((size_t)nr * k);
+        int rc = nns_batch(nullptr, nr, dix.emb_d, k, g.host ? hu.data() : nullptr, W, gi.data(), gd.data(), gn.data(), false, du, rows.data());
+        if (rc != B200_OK) return rc;
+        for (uint32_t j = 0; j < nr; j++) {
+            const uint32_t i = at[j], q = g.queries[i], id = rq->docids[q];
+            // U \ {id}: the target leaves the list wherever it is (with zero vectors or ties it need not come first)
+            std::vector<std::pair<uint32_t, float>> list;
+            for (uint32_t e = 0; e < gn[j] && list.size() < keep; e++)
+                if (gi[(size_t)j * k + e] != id) list.push_back({gi[(size_t)j * k + e], gd[(size_t)j * k + e]});
+            std::unordered_set<uint32_t> seen{id};
+            uint32_t skipped = 0, hits = 0;
+            for (const auto &c : list) {
+                if (hits == limit) break;
+                if (!seen.insert(c.first).second) continue;
+                if (skipped < offset) {
+                    skipped++;
+                    continue;
+                }
+                float sim = 1.0f - c.second;
+                if (has_distribution) sim = distribution_shift(dist_mean, dist_sigma, sim);
+                if (rq->has_ranking_score_threshold && (double)sim < rq->ranking_score_threshold) {
+                    // candidates = (candidates \ {doc}) AND seen: the documents walked before this one
+                    if (r->n_candidates) r->n_candidates[q] = seen.size() - 2;
+                    break;
+                }
+                const size_t o = (size_t)q * limit + hits++;
+                r->docids[o] = c.first;
+                if (r->n_scores) {
+                    r->n_scores[o] = 1;
+                    r->score_kind[o * B200_MAX_SCORES] = B200_S_VECTOR;
+                    r->score_rank[o * B200_MAX_SCORES] = 0;
+                    r->score_max[o * B200_MAX_SCORES] = 1;
+                    r->score_sim[o * B200_MAX_SCORES] = sim;
+                }
+            }
+            r->n_hits[q] = hits;
         }
     }
     return B200_OK;

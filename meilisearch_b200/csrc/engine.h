@@ -405,6 +405,8 @@ struct Engine {
     HostIndex hix;
     DeviceIndex dix;
     std::vector<uint64_t> emb_bitmap;  // documents owning at least one embedding
+    std::vector<uint32_t> emb_row;     // docid -> its staged row (UINT32_MAX: none); b200_similar_batch's query rows
+    bool emb_multi_row = false;        // some document owns more than one row (b200_similar_batch refuses such stores)
     uint32_t emb_d_user = 0;           // the caller's embedding dimension (rows are zero-padded to a multiple of 8 on the device)
     bool has_distribution = false;
     float dist_mean = 0, dist_sigma = 0;
@@ -466,6 +468,8 @@ struct Engine {
     DevBuf<uint32_t> d_vsel_ids, d_vsel_n;
     DevBuf<unsigned long long> d_cand, d_vruns, d_vpartial;
     DevBuf<uint16_t> d_vq16;
+    DevBuf<uint32_t> d_vrows;                      // query rows of a similar batch
+    DevBuf<unsigned long long> d_sim_addr, d_sim_word;  // a similar batch's target words of device universes
     std::vector<cudaEvent_t> ev_pool;  // pairs recorded around kernels, resolved after the step's sync
     struct Timed { int cls; size_t a, b; };
     std::vector<Timed> timed;
@@ -495,9 +499,10 @@ struct Engine {
     // sharded: every rank passes the same queries and scans its own rows; the per-shard top-k lists are all-gathered (NCCL, on the
     // vector stream) and merged on the device; every rank returns the merged result
     // dev_cand: a candidate bitmap already on the device (then `cand` is ignored)
+    // rows: the queries are these staged rows (n_q host row indices; `queries` is ignored and d must be the staged dimension): they
+    // are gathered on the device, exactly as the f32 copies of the rows would be scanned
     int nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t limit, const uint64_t *cand, uint64_t n_cand_words, uint32_t *ids_out,
-                  float *dist_out, uint32_t *n_out, bool sharded = false, const unsigned long long *dev_cand = nullptr);
-    ShardComm sc;
+                  float *dist_out, uint32_t *n_out, bool sharded = false, const unsigned long long *dev_cand = nullptr, const uint32_t *rows = nullptr);    ShardComm sc;
     DevBuf<float> d_vpart_dist;  // sliced top-k selection: per-slice candidates
     DevBuf<uint32_t> d_vpart_ids, d_vpart_n;
     DevBuf<uint32_t> d_gather_ids, d_gather_n;
@@ -528,6 +533,17 @@ struct Engine {
         std::vector<int32_t> error_leaf;                 // filter programs: the leaf whose error failed the query, -1 (may be empty)
     };
     const GeoFiltered *geo_filtered = nullptr;
+    // the queries of a vector batch grouped by filtered universe, so that each group is one scan: the caller's host bitmap (host;
+    // nullptr and dev nullptr: documents_ids) or a device bitmap of the geo / filter pre-pass (dev).  Queries the pre-pass failed
+    // are left out.  count = |documents_ids AND universe|.
+    struct UniverseGroup {
+        const uint64_t *host;
+        const unsigned long long *dev;
+        uint64_t count;
+        std::vector<uint32_t> queries;
+    };
+    std::vector<UniverseGroup> group_by_universe(uint32_t n_queries, const uint64_t *const *universes, const GeoFiltered *gf) const;
+    int similar_batch(const b200_similar_request *rq, b200_results *r);
     bool geo_filterable() const;  // b200_stage_geo_fields named both fields
     int reserve_geo_bitmaps(DevBuf<unsigned long long> &buf, size_t n_bitmaps);  // B200_ERR_CAPACITY when they do not fit
     int run_geo_filter(const std::vector<GeoClause> &clauses, const std::vector<uint32_t> &slot_clauses, std::vector<GeoSlot> &slots,

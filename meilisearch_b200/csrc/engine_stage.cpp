@@ -365,9 +365,16 @@ int Engine::stage_embeddings(const float *vectors, const uint16_t *half_rows, ui
     CU(cudaStreamSynchronize(stream), "sync");
     // which documents own an embedding (VectorSort returns the others as its last bucket, vector_sort.rs:128-160)
     emb_bitmap.assign(hix.n_words64, 0);
+    emb_row.assign(hix.n_words64 * 64, UINT32_MAX);
+    emb_multi_row = false;
     for (uint64_t r = 0; r < n; r++) {
         const uint32_t doc = docids ? docids[r] : (uint32_t)r;
         if ((doc >> 6) < emb_bitmap.size()) emb_bitmap[doc >> 6] |= 1ull << (doc & 63);
+        // rows of documents beyond the document range are scanned but never a similar query's target
+        if (doc < emb_row.size()) {
+            if (emb_row[doc] != UINT32_MAX) emb_multi_row = true;
+            emb_row[doc] = (uint32_t)r;
+        }
     }
     dix.emb_n = n;
     dix.emb_d = d;
@@ -517,11 +524,28 @@ int Engine::comm_init(int rank, int world, const uint8_t *unique_id) {
 }
 
 int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t limit, const uint64_t *cand, uint64_t n_cand_words,
-                      uint32_t *ids_out, float *dist_out, uint32_t *n_out, bool sharded, const unsigned long long *dev_cand) {
+                      uint32_t *ids_out, float *dist_out, uint32_t *n_out, bool sharded, const unsigned long long *dev_cand, const uint32_t *rows) {
     if (sharded && (!sc.comm || sc.world < 1)) return fail(B200_ERR_STATE, "sharded nns before b200_comm_init");
     CU(cudaSetDevice(device), "cudaSetDevice");
     if (!dix.emb) return fail(B200_ERR_STATE, "nns before b200_stage_embeddings");
     if (d != emb_d_user && d != dix.emb_d) return fail(B200_ERR_INVALID, "nns: query dimension differs from the staged embeddings");
+    if (rows && d != dix.emb_d) return fail(B200_ERR_INVALID, "nns: row queries take the staged dimension");
+    // the f32 queries of [q0, q0 + nq) into d_vq: copied from the host, or gathered from their staged rows (then with their inverse
+    // norms into `inv` when it is given; only the row indices cross PCIe)
+    auto load_queries = [&](uint32_t q0, uint32_t nq, float *inv) -> int {
+        if (!rows) {
+            CU(cudaMemcpyAsync(d_vq.p, queries + (size_t)q0 * d, (size_t)nq * d * 4, cudaMemcpyHostToDevice, vt.stream), "H2D queries");
+            vstats.h2d_bytes += (size_t)nq * d * 4;
+            return B200_OK;
+        }
+        CU(d_vrows.reserve(nq), "alloc query rows");
+        CU(cudaMemcpyAsync(d_vrows.p, rows + q0, (size_t)nq * 4, cudaMemcpyHostToDevice, vt.stream), "H2D query rows");
+        vstats.h2d_bytes += (size_t)nq * 4;
+        CU(launch_vec_gather_rows(vt.stream, dix.emb, d, d_vrows.p, nq, d_vq.p, inv), "vec_gather_rows");
+        vstats.kernel_launches++;
+        vstats.vector_bytes += (uint64_t)nq * d * 2;
+        return B200_OK;
+    };
     if (d != dix.emb_d) {  // rows were zero-padded at staging: pad the queries the same way
         std::vector<float> padded((size_t)n_q * dix.emb_d, 0.f);
         for (uint32_t q = 0; q < n_q; q++) memcpy(padded.data() + (size_t)q * dix.emb_d, queries + (size_t)q * d, (size_t)d * 4);
@@ -574,8 +598,7 @@ int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t l
                 CU(d_vsel_ids.reserve((size_t)n_pad * limit), "alloc selection");
                 CU(d_vsel_n.reserve(n_pad), "alloc selection");
                 float *d_qinv = d_vq.p + (size_t)nq * d;
-                CU(cudaMemcpyAsync(d_vq.p, queries + (size_t)q0 * d, (size_t)nq * d * 4, cudaMemcpyHostToDevice, vt.stream), "H2D queries");
-                vstats.h2d_bytes += (size_t)nq * d * 4;
+                if (int rc = load_queries(q0, nq, nullptr)) return rc;
                 CU(launch_vec_prep_queries(vt.stream, d_vq.p, nq, n_pad, d, d_vq16.p, d_qinv), "vec_prep_queries");
                 vstats.kernel_launches++;
                 size_t m0 = vt.mark();
@@ -628,18 +651,20 @@ int Engine::nns_batch(const float *queries, uint32_t n_q, uint32_t d, uint32_t l
     std::vector<uint32_t> sel_i((size_t)chunk * (limit + tie_cap)), sel_n((size_t)chunk * 2);
     for (uint32_t q0 = 0; q0 < n_q; q0 += chunk) {
         uint32_t nq = std::min(chunk, n_q - q0);
-        for (uint32_t q = 0; q < nq; q++) {
-            double s = 0;
-            const float *v = queries + (size_t)(q0 + q) * d;
-            for (uint32_t i = 0; i < d; i++) s += (double)v[i] * v[i];
-            float nrm = (float)std::sqrt(s);
-            qinv[q] = nrm > 0.f ? 1.0f / nrm : 0.f;
-        }
         float *d_qinv = d_vq.p + (size_t)chunk * d;
-        CU(cudaMemcpyAsync(d_vq.p, queries + (size_t)q0 * d, (size_t)nq * d * 4, cudaMemcpyHostToDevice, vt.stream), "H2D queries");
-        vstats.h2d_bytes += (size_t)nq * d * 4 + nq * 4;
+        if (int rc = load_queries(q0, nq, rows ? d_qinv : nullptr)) return rc;
+        if (!rows) {
+            for (uint32_t q = 0; q < nq; q++) {
+                double s = 0;
+                const float *v = queries + (size_t)(q0 + q) * d;
+                for (uint32_t i = 0; i < d; i++) s += (double)v[i] * v[i];
+                float nrm = (float)std::sqrt(s);
+                qinv[q] = nrm > 0.f ? 1.0f / nrm : 0.f;
+            }
+            vstats.h2d_bytes += nq * 4;
+            CU(cudaMemcpyAsync(d_qinv, qinv.data(), nq * 4, cudaMemcpyHostToDevice, vt.stream), "H2D query norms");
+        }
         vstats.d2h_bytes += (size_t)nq * (limit + tie_cap) * 8 + nq * 8;
-        CU(cudaMemcpyAsync(d_qinv, qinv.data(), nq * 4, cudaMemcpyHostToDevice, vt.stream), "H2D query norms");
         for (uint32_t t = 0; t < nq;) {
             uint32_t left = nq - t;
             int qt = left >= 8 ? 8 : (left >= 4 ? 4 : (left >= 2 ? 2 : 1));

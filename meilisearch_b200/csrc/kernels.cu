@@ -1363,6 +1363,41 @@ cudaError_t launch_emb_norm_f16(cudaStream_t s, const void *rows_fp16, float *in
     return cudaGetLastError();
 }
 
+// ---- queries that are staged rows (b200_similar_batch): one CTA per query copies its fp16 row into the f32 query buffer; with
+// `inv`, thread 0 then computes the inverse norm exactly as Engine::nns_batch does on the host for f32 queries: the squares summed in
+// double in index order (no contraction), the correctly rounded sqrt rounded to float, 1 / that in float (0 for a zero norm).  The
+// f32 values are exact copies of the fp16 ones, so a similar query and an nns query on the row's f32 copy scan the same bits.
+__global__ void __launch_bounds__(128) vec_gather_rows_kernel(const __half *__restrict__ emb, uint32_t d, const uint32_t *__restrict__ rows,
+                                                              float *__restrict__ out, float *__restrict__ inv) {
+    const __half *src = emb + (size_t)rows[blockIdx.x] * d;
+    float *dst = out + (size_t)blockIdx.x * d;
+    for (uint32_t i = threadIdx.x; i < d; i += blockDim.x) dst[i] = __half2float(src[i]);
+    if (inv && threadIdx.x == 0) {
+        double s = 0.0;
+        for (uint32_t i = 0; i < d; i++) {
+            const double v = (double)__half2float(src[i]);
+            s = __dadd_rn(s, __dmul_rn(v, v));
+        }
+        const float nrm = __double2float_rn(sqrt(s));
+        inv[blockIdx.x] = nrm > 0.f ? __fdiv_rn(1.0f, nrm) : 0.f;
+    }
+}
+cudaError_t launch_vec_gather_rows(cudaStream_t s, const void *emb_fp16, uint32_t d, const uint32_t *rows, uint32_t n, float *out, float *inv) {
+    if (!n) return cudaSuccess;
+    vec_gather_rows_kernel<<<n, 128, 0, s>>>(reinterpret_cast<const __half *>(emb_fp16), d, rows, out, inv);
+    return cudaGetLastError();
+}
+// out[i] = the u64 word at device address addr[i]
+__global__ void __launch_bounds__(256) gather_words_kernel(const unsigned long long *__restrict__ addr, uint32_t n, unsigned long long *__restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = *reinterpret_cast<const unsigned long long *>(addr[i]);
+}
+cudaError_t launch_gather_words(cudaStream_t s, const unsigned long long *addr, uint32_t n, unsigned long long *out) {
+    if (!n) return cudaSuccess;
+    gather_words_kernel<<<(n + 255) / 256, 256, 0, s>>>(addr, n, out);
+    return cudaGetLastError();
+}
+
 // ---- corpus-sharded vector stage: merge of the per-shard top-k lists after the all-gather
 // One CTA per query: the shards' runs (ascending (distance, docid), n valid entries each) become 64-bit keys
 // distance-bits << 32 | docid, are sorted by a bitonic network in shared memory, and the first `k` are written back.

@@ -67,6 +67,11 @@ __host__ __device__ inline bool norm_rule_ok(float pn) { return pn > 0.f && pn <
 // staging of the vector store: f32 rows -> fp16 rows + inverse norms; inverse norms of fp16 rows
 cudaError_t launch_emb_from_f32(cudaStream_t s, const float *in, void *out_fp16, float *inv_norm, uint64_t n, uint32_t d);
 cudaError_t launch_emb_norm_f16(cudaStream_t s, const void *rows_fp16, float *inv_norm, uint64_t n, uint32_t d);
+// queries that are staged rows: out[i * d ..] = f32 copy of row rows[i] (rows: device); inv (may be null): their inverse norms as
+// Engine::nns_batch computes them on the host for f32 queries
+cudaError_t launch_vec_gather_rows(cudaStream_t s, const void *emb_fp16, uint32_t d, const uint32_t *rows, uint32_t n, float *out, float *inv);
+// out[i] = *(u64 *)addr[i] for n device addresses (addr, out: device)
+cudaError_t launch_gather_words(cudaStream_t s, const unsigned long long *addr, uint32_t n, unsigned long long *out);
 
 // corpus-sharded vector stage: merge `world` gathered per-shard top-k lists ([shard][query][k] + [shard][query] counts) per query
 cudaError_t launch_shard_merge(cudaStream_t s, const uint32_t *g_ids, const float *g_dist, const uint32_t *g_n, uint32_t world, uint32_t n_q,
