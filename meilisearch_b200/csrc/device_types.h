@@ -204,9 +204,15 @@ struct GeoDesc {
     uint32_t bits[5];
     uint32_t lo, hi;                // hi - lo <= SORT_WINDOW
     uint32_t *dst;                  // hi - lo docids
-    double *dst_dist;               // their haversine distance to the target (metres)
     unsigned long long *dst_key;    // their rtree key
     uint32_t *info;                 // out: passes, documents collected
+    // iterative keys decided on the host (geo_math.cuh, geo_ambiguous): (docid << 32 | floor metres), ascending
+    const unsigned long long *patch;
+    uint32_t n_patch;
+    // geo_ambiguous_kernel: the documents of universe AND geo whose floor is ambiguous, the first amb_cap of them into amb, their
+    // number into *amb_count
+    uint32_t amb_cap;
+    uint32_t *amb, *amb_count;
 };
 // geo_count_kernel: |universe AND geo| per query
 struct GeoCount {
@@ -231,6 +237,11 @@ struct GeoClause {
 // the first point of the rtree order whose haversine exceeds the radius: (squared distance bits, docid); all ones = none
 struct __align__(16) GeoFirst {
     unsigned long long key, doc;
+};
+// a band point whose haversine is ambiguous against its clause's radius (geo_math.cuh), left to the host: clause, docid, rtree key
+struct GeoAmb {
+    uint32_t clause, doc;
+    unsigned long long key;
 };
 // one filtered universe: ub AND the clauses slot_clauses[c_begin, c_end) (NOT clauses complemented), written to dst, its popcount
 // added to *count

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <chrono>
 #include <condition_variable>
 #include <functional>
@@ -344,6 +345,10 @@ struct NcclId {
 
 // geo filter clause validation (engine_geo.cpp): 0, or B200_ERR_INVALID with the reference's message
 int geo_clause(uint8_t kind, uint8_t neg, const double *a, GeoClause &c, std::string &err);
+// distance_between_two_points (lib.rs:388-393) with the host's libm, as the reference computes it: NaN when a > 1 (engine_geo.cpp)
+double geo_distance_host(double t_lat, double t_lng, double p_lat, double p_lng);
+// `distance as usize`, capped at GEO_FLOOR_MAX: NaN and negatives to 0
+inline uint32_t geo_floor_host(double m) { return m > 0.0 ? (uint32_t)std::min(m, (double)GEO_FLOOR_MAX) : 0u; }
 
 struct GraphObj;  // S1: opaque query graph (engine_search.cpp)
 void free_graph(GraphObj *);
@@ -444,12 +449,13 @@ struct Engine {
     DevBuf<GeoCount> d_geo_count;
     DevBuf<GeoDesc> d_geo_desc;
     DevBuf<uint32_t> d_geo_u32;
-    DevBuf<double> d_geo_dist;
     DevBuf<unsigned long long> d_geo_key;
+    DevBuf<unsigned long long> d_geo_patch;  // the batch's iterative keys decided on the host (GeoDesc::patch)
     // geo filters (geo_filter.cu, engine_geo.cpp): the distinct clauses, their first failing points, clause ids, slots and counts;
     // the callers' universes AND documents_ids; the slots' bitmaps (n_words64 words each)
     DevBuf<GeoClause> d_gf_clause;
     DevBuf<GeoFirst> d_gf_first;
+    DevBuf<GeoAmb> d_gf_amb;  // pass 1's ambiguous band points (the count in d_gf_u32's last word)
     DevBuf<uint32_t> d_gf_u32;
     DevBuf<GeoSlot> d_gf_slot;
     DevBuf<unsigned long long> d_gf_count, d_gf_caller, d_gf_univ;

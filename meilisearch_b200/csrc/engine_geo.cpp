@@ -55,6 +55,13 @@ void geo_radius_band(double r_eps, double &lo, double &hi) {
 
 }  // namespace
 
+double geo_distance_host(double t_lat, double t_lng, double p_lat, double p_lng) {
+    const double to_rad = M_PI / 180.0;
+    const double s_lat = std::sin((p_lat - t_lat) * to_rad / 2.0), s_lng = std::sin((p_lng - t_lng) * to_rad / 2.0);
+    const double a = s_lat * s_lat + s_lng * s_lng * std::cos(t_lat * to_rad) * std::cos(p_lat * to_rad);
+    return 2.0 * std::atan2(std::sqrt(a), std::sqrt(1.0 - a)) * 6371000.0;
+}
+
 // One clause from the ABI's (kind, four doubles), validated in the reference's order: the coordinates finite, then their ranges, then
 // the radius (finite) or top >= bottom.  Returns 0 or B200_ERR_INVALID with the reference's message.
 int geo_clause(uint8_t kind, uint8_t neg, const double *a, GeoClause &c, std::string &err) {
@@ -150,6 +157,7 @@ int Engine::run_geo_filter(const std::vector<GeoClause> &clauses, const std::vec
     u32.insert(u32.end(), slot_clauses.begin(), slot_clauses.end());
     CU(d_gf_clause.reserve(clauses.size() + 1), "alloc geo clauses");
     CU(d_gf_first.reserve(clauses.size() + 1), "alloc geo clauses");
+    CU(d_gf_amb.reserve(std::max<size_t>(d_gf_amb.cap, 1024)), "alloc geo clauses");
     CU(d_gf_u32.reserve(u32.size() + 1), "alloc geo clauses");
     CU(d_gf_slot.reserve(n_slots + 1), "alloc geo slots");
     CU(d_gf_count.reserve(n_slots + 1), "alloc geo slots");
@@ -164,9 +172,40 @@ int Engine::run_geo_filter(const std::vector<GeoClause> &clauses, const std::vec
     // algorithmic bytes: each pass reads the geo bitmap and the geo documents' points once (xyz in pass 1, xyz + lat / lng in pass
     // 2); pass 2 reads each slot's universe and writes its bitmap
     if (n_radius) {
-        const size_t m0 = mark();
-        CU(launch_geo_first_fail(stream, d_geo_ub, d_geo_pts, W, d_gf_clause.p, d_gf_u32.p, n_radius, d_gf_first.p), "geo_first_fail");
-        time_kernel(B200_K_GEO_FILTER, m0, mark(), (uint64_t)W * 8 + n_geo * 24 + n_radius * (uint64_t)sizeof(GeoFirst));
+        // pass 1; the band points it cannot decide are decided here, with libm, and the failing ones folded into F (a minimum).  The
+        // list is read after the pass; when it overflowed, the pass runs again with room for all of it.
+        uint32_t *amb_count = d_gf_u32.p + u32.size();
+        uint32_t n_amb = 0;
+        for (int attempt = 0; attempt < 2; attempt++) {
+            if (attempt) CU(cudaMemsetAsync(d_gf_first.p, 0xff, clauses.size() * sizeof(GeoFirst), stream), "memset geo clauses");
+            CU(cudaMemsetAsync(amb_count, 0, 4, stream), "memset geo clauses");
+            const size_t m0 = mark();
+            CU(launch_geo_first_fail(stream, d_geo_ub, d_geo_pts, W, d_gf_clause.p, d_gf_u32.p, n_radius, d_gf_first.p, d_gf_amb.p,
+                                     (uint32_t)d_gf_amb.cap, amb_count), "geo_first_fail");
+            time_kernel(B200_K_GEO_FILTER, m0, mark(), (uint64_t)W * 8 + n_geo * 24 + n_radius * (uint64_t)sizeof(GeoFirst));
+            CU(cudaMemcpyAsync(&n_amb, amb_count, 4, cudaMemcpyDeviceToHost, stream), "D2H geo ambiguous");
+            CU(cudaStreamSynchronize(stream), "sync");
+            stats.d2h_bytes += 4;
+            if (n_amb <= d_gf_amb.cap) break;
+            CU(d_gf_amb.reserve(n_amb), "alloc geo ambiguous");
+        }
+        if (n_amb) {
+            std::vector<GeoAmb> amb(n_amb);
+            std::vector<GeoFirst> first(clauses.size());
+            CU(cudaMemcpyAsync(amb.data(), d_gf_amb.p, n_amb * sizeof(GeoAmb), cudaMemcpyDeviceToHost, stream), "D2H geo ambiguous");
+            CU(cudaMemcpyAsync(first.data(), d_gf_first.p, first.size() * sizeof(GeoFirst), cudaMemcpyDeviceToHost, stream), "D2H geo ambiguous");
+            CU(cudaStreamSynchronize(stream), "sync");
+            stats.d2h_bytes += n_amb * sizeof(GeoAmb) + first.size() * sizeof(GeoFirst);
+            for (const GeoAmb &x : amb) {
+                const GeoClause &k = clauses[x.clause];
+                if (geo_distance_host(k.t_lat, k.t_lng, hix.geo.lat[x.doc], hix.geo.lng[x.doc]) <= k.r_eps) continue;
+                GeoFirst &f = first[x.clause];
+                if (x.key < f.key || (x.key == f.key && x.doc < f.doc)) f = GeoFirst{x.key, x.doc};
+            }
+            CU(cudaMemcpyAsync(d_gf_first.p, first.data(), first.size() * sizeof(GeoFirst), cudaMemcpyHostToDevice, stream), "H2D geo clauses");
+            CU(cudaStreamSynchronize(stream), "sync");  // `first` is pageable and local
+            stats.h2d_bytes += first.size() * sizeof(GeoFirst);
+        }
     }
     const size_t m1 = mark();
     CU(launch_geo_filter(stream, d_geo_ub, d_geo_pts, W, d_gf_clause.p, d_gf_first.p, d_gf_u32.p + n_radius, d_gf_slot.p, n_slots), "geo_filter");

@@ -473,7 +473,11 @@ struct QState {
     unsigned long long geo_split_key = 0;
     uint32_t geo_split_doc = 0;
     std::vector<uint32_t> geo_docs;
-    std::vector<double> geo_dist;
+    std::vector<double> geo_dist;  // computed on the host (geo_distance_host), as the chain compares them
+    // the iterative keys the device cannot decide, decided on the host: (docid << 32 | floor metres), ascending; listed once, the
+    // first time a window of the query reaches its iterative part
+    bool geo_patched = false;
+    std::vector<unsigned long long> geo_patch;
     // arena blocks of levels bucket_sort has left; the lane's driver returns them to its allocator at the start of its next step
     // (the emissions queued by the same advance() still read them: they run first on the lane's stream, before any new owner writes)
     std::vector<std::pair<size_t, size_t>> freed;
@@ -3260,10 +3264,82 @@ struct KeywordBatch {
         for (uint32_t s = 0; s < have;) {
             const double d0 = q.geo_dist[s];
             uint32_t e = s + 1;
-            while (e < have && e - s < cap && std::fabs(d0 - q.geo_dist[e]) <= GEO_MARGIN_M) e++;
+            // `(d0 - d).abs() > margin` ends the bucket (documents/geo_sort.rs:177-180): a NaN distance joins it
+            while (e < have && e - s < cap && !(std::fabs(d0 - q.geo_dist[e]) > GEO_MARGIN_M)) e++;
             ends.push_back(e);
             s = e;
         }
+    }
+    // The iterative keys of the queries whose windows first reach their iterative part in this round (descs in mode 1 or 2): the
+    // documents geo_ambiguous_kernel lists are decided with libm into the query's patch.  Then every window gets its query's patch.
+    int geo_patches(std::vector<GeoDesc> &descs, const std::vector<std::pair<uint32_t, bool>> &owner) {
+        std::vector<uint32_t> fresh;  // one window per query to list
+        for (size_t k = 0; k < descs.size(); k++) {
+            QState &q = *qs[owner[k].first];
+            if (descs[k].mode == 0 || q.geo_patched) continue;
+            q.geo_patched = true;
+            fresh.push_back((uint32_t)k);
+        }
+        if (!fresh.empty()) {
+            const uint32_t nf = (uint32_t)fresh.size();
+            uint32_t cap = 1024;
+            std::vector<uint32_t> count(nf);
+            for (int attempt = 0; attempt < 2; attempt++) {
+                std::vector<GeoDesc> ds(nf);
+                CU(eng.d_geo_u32.reserve((size_t)nf * (cap + 1)), "alloc geo ambiguous");
+                CU(eng.d_geo_desc.reserve(nf), "alloc geo ambiguous");
+                for (uint32_t f = 0; f < nf; f++) {
+                    ds[f] = descs[fresh[f]];
+                    ds[f].amb_cap = cap;
+                    ds[f].amb = eng.d_geo_u32.p + nf + (size_t)f * cap;
+                    ds[f].amb_count = eng.d_geo_u32.p + f;
+                }
+                CU(cudaMemsetAsync(eng.d_geo_u32.p, 0, nf * 4, eng.stream), "memset geo ambiguous");
+                CU(cudaMemcpyAsync(eng.d_geo_desc.p, ds.data(), nf * sizeof(GeoDesc), cudaMemcpyHostToDevice, eng.stream), "H2D geo ambiguous");
+                const size_t m0 = eng.mark();
+                CU(launch_geo_ambiguous(eng.stream, eng.d_geo_desc.p, nf), "geo_ambiguous");
+                eng.time_kernel(B200_K_GEO, m0, eng.mark(), 0);
+                CU(cudaMemcpyAsync(count.data(), eng.d_geo_u32.p, nf * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H geo ambiguous");
+                CU(cudaStreamSynchronize(eng.stream), "sync geo ambiguous");
+                stats.h2d_bytes += nf * sizeof(GeoDesc);
+                stats.d2h_bytes += nf * 4;
+                const uint32_t most = *std::max_element(count.begin(), count.end());
+                if (most <= cap) break;
+                cap = most;
+            }
+            std::vector<uint32_t> amb((size_t)nf * cap);
+            CU(cudaMemcpyAsync(amb.data(), eng.d_geo_u32.p + nf, amb.size() * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H geo ambiguous");
+            CU(cudaStreamSynchronize(eng.stream), "sync geo ambiguous");
+            stats.d2h_bytes += amb.size() * 4;
+            for (uint32_t f = 0; f < nf; f++) {
+                QState &q = *qs[owner[fresh[f]].first];
+                const SortRule &rule = q.sort_rules[0];
+                for (uint32_t j = 0; j < count[f]; j++) {
+                    const uint32_t doc = amb[(size_t)f * cap + j];
+                    const uint32_t m = geo_floor_host(geo_distance_host(rule.lat, rule.lng, hix.geo.lat[doc], hix.geo.lng[doc]));
+                    q.geo_patch.push_back((unsigned long long)doc << 32 | m);
+                }
+                std::sort(q.geo_patch.begin(), q.geo_patch.end());
+            }
+        }
+        std::vector<unsigned long long> all;
+        std::map<uint32_t, size_t> at;  // query -> offset of its patch in `all`
+        for (size_t k = 0; k < descs.size(); k++) {
+            const QState &q = *qs[owner[k].first];
+            if (descs[k].mode == 0 || q.geo_patch.empty()) continue;
+            auto it = at.emplace(owner[k].first, all.size());
+            if (it.second) all.insert(all.end(), q.geo_patch.begin(), q.geo_patch.end());
+            descs[k].patch = reinterpret_cast<const unsigned long long *>((uintptr_t)it.first->second);  // offsets, made pointers below
+            descs[k].n_patch = (uint32_t)q.geo_patch.size();
+        }
+        if (all.empty()) return B200_OK;
+        CU(eng.d_geo_patch.reserve(all.size()), "alloc geo patch");
+        CU(cudaMemcpyAsync(eng.d_geo_patch.p, all.data(), all.size() * 8, cudaMemcpyHostToDevice, eng.stream), "H2D geo patch");
+        CU(cudaStreamSynchronize(eng.stream), "sync geo patch");  // `all` is pageable and local
+        stats.h2d_bytes += all.size() * 8;
+        for (GeoDesc &d : descs)
+            if (d.n_patch) d.patch = eng.d_geo_patch.p + (uintptr_t)d.patch;
+        return B200_OK;
     }
     int geo_windows() {
         const GeoParams gp{b->geo_strategy, b->geo_cache_size ? b->geo_cache_size : 1000u,
@@ -3367,14 +3443,14 @@ struct KeywordBatch {
                 }
             }
             const size_t n = descs.size();
+            int rc = geo_patches(descs, owner);
+            if (rc != B200_OK) return rc;
             CU(eng.d_geo_desc.reserve(n), "alloc geo windows");
             CU(eng.d_geo_u32.reserve(rows + 2 * n), "alloc geo rows");
-            CU(eng.d_geo_dist.reserve(rows), "alloc geo rows");
             CU(eng.d_geo_key.reserve(rows), "alloc geo rows");
             for (size_t k = 0; k < n; k++) {
                 const size_t off = (uintptr_t)descs[k].dst;
                 descs[k].dst = eng.d_geo_u32.p + off;
-                descs[k].dst_dist = eng.d_geo_dist.p + off;
                 descs[k].dst_key = eng.d_geo_key.p + off;
                 descs[k].info = eng.d_geo_u32.p + rows + 2 * k;
             }
@@ -3383,21 +3459,20 @@ struct KeywordBatch {
             CU(launch_geo_window(eng.stream, eng.d_geo_desc.p, (uint32_t)n), "geo_window");
             eng.time_kernel(B200_K_GEO, m0, eng.mark(), 0);
             std::vector<uint32_t> u32(rows + 2 * n);
-            std::vector<double> dist(rows);
             std::vector<unsigned long long> key(rows);
             CU(cudaMemcpyAsync(u32.data(), eng.d_geo_u32.p, u32.size() * 4, cudaMemcpyDeviceToHost, eng.stream), "D2H geo rows");
-            CU(cudaMemcpyAsync(dist.data(), eng.d_geo_dist.p, rows * 8, cudaMemcpyDeviceToHost, eng.stream), "D2H geo rows");
             CU(cudaMemcpyAsync(key.data(), eng.d_geo_key.p, rows * 8, cudaMemcpyDeviceToHost, eng.stream), "D2H geo rows");
             CU(cudaStreamSynchronize(eng.stream), "sync geo rows");
             eng.resolve_timers();
             stats.h2d_bytes += n * sizeof(GeoDesc);
-            stats.d2h_bytes += u32.size() * 4 + rows * 16;
+            stats.d2h_bytes += u32.size() * 4 + rows * 8;
+            std::vector<size_t> dist_at(n, SIZE_MAX);  // per window: where its rows' distances go in its query's geo_dist
             for (size_t k = 0; k < n; k++) {
                 QState &q = *qs[owner[k].first];
                 const GeoDesc &d = descs[k];
                 const size_t off = d.dst - eng.d_geo_u32.p, nr = d.hi - d.lo;
                 // algorithmic bytes: every pass reads the two bitmaps and a GeoPoint per document of G; the rows are written out
-                stats.kernel_bytes[B200_K_GEO] += (uint64_t)u32[rows + 2 * k] * (W * 16ull + q.geo_n * (uint64_t)sizeof(GeoPoint)) + nr * 20ull;
+                stats.kernel_bytes[B200_K_GEO] += (uint64_t)u32[rows + 2 * k] * (W * 16ull + q.geo_n * (uint64_t)sizeof(GeoPoint)) + nr * 12ull;
                 if (u32[rows + 2 * k + 1] != nr) {
                     q.status = B200_ERR_CUDA;
                     q.error = "internal: geo window collected a different number of documents than its rank range";
@@ -3410,8 +3485,18 @@ struct KeywordBatch {
                     continue;
                 }
                 q.geo_docs.insert(q.geo_docs.end(), u32.begin() + off, u32.begin() + off + nr);
-                q.geo_dist.insert(q.geo_dist.end(), dist.begin() + off, dist.begin() + off + nr);
+                dist_at[k] = q.geo_dist.size();
+                q.geo_dist.resize(q.geo_dist.size() + nr);
             }
+            // the chain's distances, with libm as the reference computes them (windows write disjoint ranges)
+            pfor(n, [&](size_t k) {
+                if (dist_at[k] == SIZE_MAX) return;
+                QState &q = *qs[owner[k].first];
+                const SortRule &rule = q.sort_rules[0];
+                const uint32_t *docs = u32.data() + (descs[k].dst - eng.d_geo_u32.p);
+                for (uint32_t r = 0; r < descs[k].hi - descs[k].lo; r++)
+                    q.geo_dist[dist_at[k] + r] = geo_distance_host(rule.lat, rule.lng, hix.geo.lat[docs[r]], hix.geo.lng[docs[r]]);
+            });
             std::vector<uint32_t> next, ends;
             for (uint32_t i : active) {
                 QState &q = *qs[i];

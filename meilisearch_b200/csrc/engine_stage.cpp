@@ -106,10 +106,11 @@ Engine::~Engine() {
     d_geo_count.release();
     d_geo_desc.release();
     d_geo_u32.release();
-    d_geo_dist.release();
+    d_geo_patch.release();
     d_geo_key.release();
     d_gf_clause.release();
     d_gf_first.release();
+    d_gf_amb.release();
     d_gf_u32.release();
     d_gf_slot.release();
     d_gf_count.release();
@@ -277,8 +278,8 @@ int Engine::stage_finish() {
         CU(upload(&d_geo_pts, pts.data(), pts.size()), "upload geo points");
         CU(upload(&d_geo_ub, reinterpret_cast<const unsigned long long *>(g.ub.data()), g.ub.size()), "upload geo bitmap");
         stats.hbm_bytes_staged += pts.size() * sizeof(GeoPoint) + g.ub.size() * 8;
-        std::vector<double>().swap(g.lat);
-        std::vector<double>().swap(g.lng);
+        // lat / lng stay on the host: the decisions the device leaves ambiguous, and the distances of the GeoSort chain, are taken
+        // there with libm (geo_distance_host)
     }
     // release the raw staging copies
     for (auto &db : raw_dbs) {

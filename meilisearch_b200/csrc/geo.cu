@@ -6,7 +6,8 @@
 //   rtree:     squared Euclidean distance between lat_lng_to_xyz of the point and of the target (its antipode when descending), as
 //              rstar's nearest_neighbor_iter ranks points (((dx*dx) + dy*dy) + dz*dz); ties by docid;
 //   iterative: floor of the haversine distance (geoutils, R = 6371000 m), a stable sort by docid; reversed when descending.
-// The distances are those of geo_math.cuh.
+// The distances are those of geo_math.cuh.  A floor the device cannot decide (geo_ambiguous) comes from the host's patch: the
+// documents are listed by geo_ambiguous_kernel before the windows are selected.
 #include <cuda_runtime.h>
 
 #include "device_types.h"
@@ -17,7 +18,21 @@ namespace b200 {
 
 namespace {
 
-__device__ __forceinline__ uint32_t floor_m(double m) { return (uint32_t)min(m, (double)GEO_FLOOR_MAX); }
+// the iterative key: floor metres, or the host's where the device's distance is ambiguous
+__device__ __forceinline__ uint32_t iterative_floor(const GeoDesc &d, uint32_t doc, const GeoPoint &p) {
+    const GeoDist g = geo_dist(d.t_lat, d.t_lng, d.t_cos_lat, p.lat, p.lng, p.cos_lat);
+    uint32_t f = floor_m(g.m);
+    if (d.n_patch && geo_ambiguous(g, floor_threshold(g.m))) {
+        uint32_t lo = 0, hi = d.n_patch;
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi) / 2;
+            if ((uint32_t)(d.patch[mid] >> 32) < doc) lo = mid + 1;
+            else hi = mid;
+        }
+        if (lo < d.n_patch && (uint32_t)(d.patch[lo] >> 32) == doc) f = (uint32_t)d.patch[lo];
+    }
+    return f;
+}
 
 struct GeoView {
     static constexpr int THREADS = 512;
@@ -43,7 +58,7 @@ struct GeoView {
             case 1: return it ? 0u : (uint32_t)(key >> 32);
             case 2: {
                 if (!it) return (uint32_t)key;
-                const uint32_t f = floor_m(haversine_m(d.t_lat, d.t_lng, d.t_cos_lat, p));
+                const uint32_t f = iterative_floor(d, doc, p);
                 return d.asc ? f : GEO_FLOOR_MAX - f;
             }
             default: return it && !d.asc ? d.doc_max - doc : 0u;
@@ -62,7 +77,6 @@ struct GeoView {
     __device__ void emit(uint32_t i, uint32_t doc) const {
         const GeoPoint p = d.pts[doc];
         d.dst[i] = doc;
-        d.dst_dist[i] = haversine_m(d.t_lat, d.t_lng, d.t_cos_lat, p);
         d.dst_key[i] = rtree_key(d.q, p);
     }
 };
@@ -72,6 +86,19 @@ __global__ void __launch_bounds__(GeoView::THREADS) geo_window_kernel(const GeoD
     tsel::SelShared &s = *reinterpret_cast<tsel::SelShared *>(smem_raw);
     const GeoView v(descs[blockIdx.x]);
     tsel::window(v, s);
+}
+
+// The documents of universe AND geo whose floor metres the device cannot decide, for the host to decide (one CTA per descriptor).
+__global__ void __launch_bounds__(GeoView::THREADS) geo_ambiguous_kernel(const GeoDesc *__restrict__ descs, uint32_t n_descs) {
+    const GeoDesc &d = descs[blockIdx.x];
+    const GeoView v(d);
+    v.for_each_doc([&](uint32_t doc) {
+        const GeoPoint p = d.pts[doc];
+        const GeoDist g = geo_dist(d.t_lat, d.t_lng, d.t_cos_lat, p.lat, p.lng, p.cos_lat);
+        if (!geo_ambiguous(g, floor_threshold(g.m))) return;
+        const uint32_t k = atomicAdd(d.amb_count, 1u);
+        if (k < d.amb_cap) d.amb[k] = doc;
+    });
 }
 
 constexpr int COUNT_THREADS = 512;
@@ -96,6 +123,12 @@ __global__ void __launch_bounds__(COUNT_THREADS) geo_count_kernel(const GeoCount
 cudaError_t launch_geo_count(cudaStream_t s, const GeoCount *counts, uint32_t n) {
     if (!n) return cudaSuccess;
     geo_count_kernel<<<n, COUNT_THREADS, 0, s>>>(counts, n);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_geo_ambiguous(cudaStream_t s, const GeoDesc *descs, uint32_t n_descs) {
+    if (!n_descs) return cudaSuccess;
+    geo_ambiguous_kernel<<<n_descs, GeoView::THREADS, 0, s>>>(descs, n_descs);
     return cudaGetLastError();
 }
 

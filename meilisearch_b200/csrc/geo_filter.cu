@@ -34,12 +34,14 @@ __device__ void first_min(GeoFirst *dst, unsigned long long key, unsigned long l
 }
 
 // Pass 1.  One warp per clause at a time; a lane takes every 32nd document of the tile.  A point is decided by its squared chord d2
-// alone unless lo <= d2 <= hi (the band, set on the host by geo_radius_band), where the haversine is computed.  Among the points
-// that fail, the lane keeps the smallest (d2, docid): documents come in ascending docid order, so a strict `<` on d2 keeps the
-// smallest docid of a tie.
+// alone unless lo <= d2 <= hi (the band, set on the host by geo_radius_band), where the haversine is computed; a haversine the
+// device cannot place against the radius (geo_ambiguous) is listed for the host and passes here.  Among the points that fail, the
+// lane keeps the smallest (d2, docid): documents come in ascending docid order, so a strict `<` on d2 keeps the smallest docid of a
+// tie.
 __global__ void __launch_bounds__(THREADS) geo_first_fail_kernel(const unsigned long long *__restrict__ geo, const GeoPoint *__restrict__ pts,
                                                                  uint32_t n_words, const GeoClause *__restrict__ clauses,
-                                                                 const uint32_t *__restrict__ radius, uint32_t n_radius, GeoFirst *first) {
+                                                                 const uint32_t *__restrict__ radius, uint32_t n_radius, GeoFirst *first,
+                                                                 GeoAmb *amb, uint32_t amb_cap, uint32_t *amb_count) {
     __shared__ double sx[TILE_DOCS], sy[TILE_DOCS], sz[TILE_DOCS];
     __shared__ unsigned long long sgeo[GEO_FILTER_TILE_WORDS];
     const uint32_t w0 = blockIdx.x * GEO_FILTER_TILE_WORDS, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -67,7 +69,13 @@ __global__ void __launch_bounds__(THREADS) geo_first_fail_kernel(const unsigned 
             const uint32_t doc = w0 * 64 + i;
             if (d2 <= hi) {
                 const GeoPoint &p = pts[doc];
-                if (haversine_m(k.t_lat, k.t_lng, k.t_cos_lat, p.lat, p.lng, p.cos_lat) <= r_eps) continue;
+                const GeoDist g = geo_dist(k.t_lat, k.t_lng, k.t_cos_lat, p.lat, p.lng, p.cos_lat);
+                if (geo_ambiguous(g, r_eps)) {
+                    const uint32_t a = atomicAdd(amb_count, 1u);
+                    if (a < amb_cap) amb[a] = GeoAmb{radius[c], doc, key};
+                    continue;
+                }
+                if (g.m <= r_eps) continue;
             }
             best = key;
             best_doc = doc;
@@ -154,10 +162,11 @@ __global__ void __launch_bounds__(THREADS) geo_filter_kernel(const unsigned long
 }  // namespace
 
 cudaError_t launch_geo_first_fail(cudaStream_t s, const unsigned long long *geo, const GeoPoint *pts, uint32_t n_words, const GeoClause *clauses,
-                                  const uint32_t *radius, uint32_t n_radius, GeoFirst *first) {
+                                  const uint32_t *radius, uint32_t n_radius, GeoFirst *first, GeoAmb *amb, uint32_t amb_cap,
+                                  uint32_t *amb_count) {
     if (!n_radius || !n_words) return cudaSuccess;
     const uint32_t tiles = (n_words + GEO_FILTER_TILE_WORDS - 1) / GEO_FILTER_TILE_WORDS;
-    geo_first_fail_kernel<<<tiles, THREADS, 0, s>>>(geo, pts, n_words, clauses, radius, n_radius, first);
+    geo_first_fail_kernel<<<tiles, THREADS, 0, s>>>(geo, pts, n_words, clauses, radius, n_radius, first, amb, amb_cap, amb_count);
     return cudaGetLastError();
 }
 

@@ -30,13 +30,17 @@ cudaError_t launch_walk(cudaStream_t s, int cls, const TileDesc *tiles, uint32_t
 cudaError_t launch_emit(cudaStream_t s, const EmitDesc *emits, uint32_t n_emits);
 // sort.cu: one CTA per window (SortDesc)
 cudaError_t launch_sort_window(cudaStream_t s, const SortDesc *descs, uint32_t n_descs);
-// geo.cu: |universe AND geo| per query (one CTA each); one CTA per window of a GeoSort order (GeoDesc)
+// geo.cu: |universe AND geo| per query (one CTA each); the documents whose iterative key is ambiguous (one CTA per GeoDesc,
+// *amb_count zero at launch); one CTA per window of a GeoSort order (GeoDesc)
 cudaError_t launch_geo_count(cudaStream_t s, const GeoCount *counts, uint32_t n);
+cudaError_t launch_geo_ambiguous(cudaStream_t s, const GeoDesc *descs, uint32_t n_descs);
 cudaError_t launch_geo_window(cudaStream_t s, const GeoDesc *descs, uint32_t n_descs);
-// geo_filter.cu: pass 1, the first failing point of every radius clause in `radius` (first[] all ones at launch); pass 2, the slots
+// geo_filter.cu: pass 1, the first failing point of every radius clause in `radius` (first[] all ones and *amb_count zero at launch;
+// band points whose haversine is ambiguous are left out of first[] and listed, the first amb_cap into amb); pass 2, the slots
 // (counts zero at launch).  Both stage GEO_FILTER_TILE_WORDS words of points per CTA and loop over the clauses / slots.
 cudaError_t launch_geo_first_fail(cudaStream_t s, const unsigned long long *geo, const GeoPoint *pts, uint32_t n_words, const GeoClause *clauses,
-                                  const uint32_t *radius, uint32_t n_radius, GeoFirst *first);
+                                  const uint32_t *radius, uint32_t n_radius, GeoFirst *first, GeoAmb *amb, uint32_t amb_cap,
+                                  uint32_t *amb_count);
 cudaError_t launch_geo_filter(cudaStream_t s, const unsigned long long *geo, const GeoPoint *pts, uint32_t n_words, const GeoClause *clauses,
                               const GeoFirst *first, const uint32_t *slot_clauses, const GeoSlot *slots, uint32_t n_slots);
 // filter.cu: every slot's filtered universe (FilterSlot: counts and flags zero at launch); docs = documents_ids

@@ -18,13 +18,30 @@ from tests.sort_spec import sort_buckets
 GEO_STRATEGIES = ("dynamic", "iterative", "rtree")
 
 
-def distance_between_two_points(a, b):
-    """Location::haversine_distance_to (geoutils) in metres, from a to b"""
+def f64_sqrt(x):
+    """f64::sqrt: NaN for a negative number (or NaN) instead of a domain error"""
+    return math.sqrt(x) if x >= 0.0 else math.nan
+
+
+def haversine_a(a, b):
+    """the haversine's `a` term, as geoutils rounds it; it exceeds 1 by an ULP for some antipodal pairs"""
     d_lat = math.radians(b[0] - a[0])
     d_lon = math.radians(b[1] - a[1])
     lat1, lat2 = math.radians(a[0]), math.radians(b[0])
-    x = math.sin(d_lat / 2.0) * math.sin(d_lat / 2.0) + math.sin(d_lon / 2.0) * math.sin(d_lon / 2.0) * math.cos(lat1) * math.cos(lat2)
-    return 2.0 * math.atan2(math.sqrt(x), math.sqrt(1.0 - x)) * 6371000.0
+    return math.sin(d_lat / 2.0) * math.sin(d_lat / 2.0) + math.sin(d_lon / 2.0) * math.sin(d_lon / 2.0) * math.cos(lat1) * math.cos(lat2)
+
+
+def distance_between_two_points(a, b):
+    """Location::haversine_distance_to (geoutils) in metres, from a to b, with f64 semantics: a > 1 gives NaN"""
+    x = haversine_a(a, b)
+    return 2.0 * math.atan2(f64_sqrt(x), f64_sqrt(1.0 - x)) * 6371000.0
+
+
+def as_usize(d):
+    """Rust's `d as usize` on an f64: truncation, saturating at 0 (negatives, NaN) and at usize::MAX"""
+    if math.isnan(d) or d <= 0.0:
+        return 0
+    return min(int(d), 2 ** 64 - 1)
 
 
 def lat_lng_to_xyz(p):
@@ -90,7 +107,7 @@ class GeoSort:
                             break
         else:
             documents = [(d, self.gix.points[d]) for d in sorted(geo_candidates)]
-            documents.sort(key=lambda x: int(distance_between_two_points(self.point, x[1])))  # stable: docid order within a metre
+            documents.sort(key=lambda x: as_usize(distance_between_two_points(self.point, x[1])))  # stable: docid order within a metre
             cache.extend(documents)
 
     def start_iteration(self, universe):
@@ -240,5 +257,5 @@ def order_model(gix, target, ascending, universe, strategy="dynamic", cache_size
     q = lat_lng_to_xyz(target if ascending else opposite_of(target))
     rt = sorted(g, key=lambda d: (distance_2(gix.xyz[d], q), d))
     head, tail = rt[:m], sorted(rt[m:])
-    tail.sort(key=lambda d: int(distance_between_two_points(target, gix.points[d])))
+    tail.sort(key=lambda d: as_usize(distance_between_two_points(target, gix.points[d])))
     return head + (tail if ascending else tail[::-1])
